@@ -1,4 +1,4 @@
-"""aurora_b200 — Blackwell (sm_100a) implementation of Aurora's forward pass behind the reference's API
+"""aurora_b200 — Hopper (H100, sm_90a) implementation of Aurora's forward pass behind the reference's API
 (`aurora/__init__.py:3-30`): ``Aurora*`` model classes, ``Batch``, ``Metadata`` and ``rollout``."""
 
 from aurora_b200.batch import Batch, Metadata

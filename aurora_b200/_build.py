@@ -1,4 +1,4 @@
-"""In-tree build of ``libaurora_b200.so`` (sm_100a only) with plain ``nvcc``.
+"""In-tree build of ``libaurora_b200.so`` (sm_90a only) with plain ``nvcc``.
 
 The shared library lands next to the sources (``aurora_b200/csrc/libaurora_b200.so``) so that it
 travels with a snapshot of the repository; objects go to ``build/`` (git-ignored).  Nothing here
@@ -21,7 +21,7 @@ OBJ_DIR = ROOT / "build" / "obj"
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-O3",
     "-std=c++17",
     "-lineinfo",
@@ -68,7 +68,7 @@ def is_stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) -> Path:
-    """Compile every ``csrc/*.cu`` for sm_100a and link ``libaurora_b200.so``."""
+    """Compile every ``csrc/*.cu`` for sm_90a and link ``libaurora_b200.so``."""
     if not force and not is_stale():
         return LIB_PATH
     nvcc = _nvcc()
@@ -100,7 +100,7 @@ def build(force: bool = False, verbose: bool = False, ptxas_info: bool = False) 
                 print(f"--- {obj.name}\n{log}")
     objs = [str(o) for o, _ in results]
     tmp = LIB_PATH.with_suffix(".so.tmp")
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(tmp), *objs]
+    cmd = [nvcc, "-shared", *NVCC_FLAGS[:2], "-o", str(tmp), *objs]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

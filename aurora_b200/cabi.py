@@ -192,7 +192,7 @@ def gemm(
     act: int = AB_ACT_NONE,
     peer_push=None,
 ) -> None:
-    """``out = act(a @ w.T + bias) + residual`` on the tcgen05 GEMM (a, w bf16; outputs preallocated).
+    """``out = act(a @ w.T + bias) + residual`` on the wgmma GEMM (a, w bf16; outputs preallocated).
     `peer_push` (an `AbHaloPush`): the epilogue also stores the boundary rows it names into neighbouring GPUs' memory."""
     assert a.dtype == w.dtype, (a.dtype, w.dtype)
     m, k = a.shape

@@ -1,7 +1,7 @@
 // Whole-block entry point: one call runs a complete Swin3DTransformerBlock (aurora/model/swin3d.py:440-509) on the
 // flat token stream — what the reference does in ~40 ATen / cuBLAS / SDPA calls per block:
 //
-//   qkv   = x_b16 · Wqkv^T + b                      (tcgen05 GEMM; LoRA already merged into Wqkv, lora.py:104-129)
+//   qkv   = x_b16 · Wqkv^T + b                      (wgmma GEMM; LoRA already merged into Wqkv, lora.py:104-129)
 //   [latitude slab: push K | V halo rows to the neighbours, wait for theirs            csrc/halo.cu]
 //   att   = shifted-window attention(qkv)           (roll / pad / partition / mask / SDPA / reverse / crop / un-roll)
 //   y     = att · Wproj^T + b

@@ -1,15 +1,17 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a:  out = act(A · Wᵀ + bias) + residual.
+// Persistent, warp-specialised wgmma GEMM for sm_90a:  out = act(A · Wᵀ + bias) + residual.
 //
 //   A [M,K] bf16 (K contiguous), W [N,K] bf16 (K contiguous, nn.Linear layout), fp32 accumulation.
 //
-//   warp 0      : TMA producer   (one lane) — 128B-swizzled {64 x 128} A tiles and {64 x BN} W tiles
-//   warp 1      : MMA issuer     (one lane) — tcgen05.mma.cta_group::1.kind::f16, M=128, N=BN, K=16
-//   warp 2      : TMEM allocator (2 x BN fp32 columns: double-buffered accumulator)
-//   warps 4..11 : epilogue       — tcgen05.ld TMEM->registers, bias / erf-GELU / residual, stores
+//   warpgroup 0    : TMA producer (one lane) — 128B-swizzled {64 x 128} A tiles and {64 x BN} W tiles into a ring of
+//                    shared-memory stages; gives its registers up (setmaxnreg) to the math warpgroups
+//   warpgroups 1-2 : math + epilogue — each owns 64 of the tile's 128 rows: wgmma.mma_async m64nBNk16 straight from the
+//                    swizzled stages, the 64 x BN fp32 accumulator in registers; bias / erf-GELU / residual on the
+//                    registers, 16-bit-only outputs through swizzled shared memory and a TMA store
 //
-// Three pipelines: smem full/empty (TMA <-> MMA), TMEM full/empty (MMA <-> epilogue) and the static
-// persistent tile schedule (tile = blockIdx.x + i * gridDim.x, N-blocks fastest so that the CTAs
-// running concurrently share the same A rows in L2 while W stays L2-resident).
+// Pipelines: full / empty mbarriers per stage (TMA <-> wgmma) and the static persistent tile schedule
+// (tile = blockIdx.x + i * gridDim.x, N-blocks fastest so that the CTAs running concurrently share the same A rows in
+// L2 while W stays L2-resident).  One wgmma group stays in flight while the next stage is waited for; while the math
+// warpgroups run a tile's epilogue the producer already fills the ring with the next tile's operands.
 //
 // Replaces: every nn.Linear on Aurora's forward path (see include/aurora_b200.h).
 #include <stdlib.h>
@@ -17,14 +19,16 @@
 
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace ab {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 bytes = one swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kNumEpiWarps = 8;
-constexpr int kNumThreads = 128 + kNumEpiWarps * 32;
+constexpr int kWgmmaK = 16;
+constexpr int kMathWarps = 8;  // two warpgroups x 64 rows
+constexpr int kNumThreads = 128 + kMathWarps * 32;
+constexpr int kBoxRows = 16;   // rows of one epilogue box = rows of the accumulator one warp holds
 
 template <int BN>
 struct GemmCfg {
@@ -32,12 +36,11 @@ struct GemmCfg {
   static constexpr int kStageBytesB = BN * kBlockK * 2;
   static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
   static constexpr int kStages = BN >= 256 ? 4 : (BN >= 128 ? 6 : 8);
-  static constexpr uint32_t kTmemCols = 2 * BN;  // two accumulator stages
   static constexpr int kBarrierBytes = 256;
-  static constexpr int kStagingBytes = kNumEpiWarps * 4096;  // one 32-row x 128-byte store box per epilogue warp
+  static constexpr int kStagingBytes = kMathWarps * kBoxRows * 128;  // one 16-row x 128-byte store box per math warp
   static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBarrierBytes + 1024;  // +1024: alignment
-  static_assert((kTmemCols & (kTmemCols - 1)) == 0 && kTmemCols >= 32 && kTmemCols <= 512, "TMEM columns");
-  static_assert((2 * kStages + 4) * 8 + 4 <= kBarrierBytes, "barrier area");
+  static_assert(2 * kStages * 8 <= kBarrierBytes, "barrier area");
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 };
 
 // Rows of the 16-bit output that are ALSO stored into a neighbouring GPU's memory by the epilogue (the K | V halo rows of
@@ -47,7 +50,7 @@ struct PeerRows {
   int n_ranges;         // 0 = off
   int col_from;         // only boxes whose first column is >= col_from are sent (multiple of 64)
   int dst_ld;           // destination row pitch in elements
-  int expected;         // number of 32-row x 64-column epilogue boxes of this launch that carry peer rows
+  int expected;         // number of 16-row x 64-column epilogue boxes of this launch that carry peer rows
   int row_begin[8], row_end[8];
   uint16_t* dst[8];     // peer address of (row_begin[i], col_from)
   uint32_t* flag[2];    // the neighbours' "rows landed" flags
@@ -68,7 +71,7 @@ struct GemmArgs {
   PeerRows peer;
 };
 
-// This lane's destination in a neighbour's memory for the box (rows row0 + lane, columns col .. col + 64), or nullptr.
+// Destination in a neighbour's memory of columns col .. col + 64 of output row `row`, or nullptr.
 __device__ __forceinline__ uint16_t* peer_row_ptr(const GemmArgs& g, int row, int col) {
   uint16_t* p = nullptr;
   if (g.peer.n_ranges > 0 && col >= g.peer.col_from && row < g.m) {
@@ -98,125 +101,112 @@ __device__ __forceinline__ void peer_box_done(const GemmArgs& g, int lane) {
   }
 }
 
+// Bias and activation on two adjacent accumulator columns (col, col + 1; col is even).
+__device__ __forceinline__ void bias_act2(const GemmArgs& g, int col, float& x0, float& x1) {
+  if (g.bias != nullptr) {
+    if (col + 1 < g.n) {
+      x0 += __ldg(g.bias + col);
+      x1 += __ldg(g.bias + col + 1);
+    } else if (col < g.n) {
+      x0 += __ldg(g.bias + col);
+    }
+  }
+  if (g.act == AB_ACT_GELU_ERF) {
+    x0 = gelu_erf(x0);
+    x1 = gelu_erf(x1);
+  }
+}
+
+// General epilogue: this thread's two rows (row0, row0 + 8) x BN / 4 columns of the accumulator straight to global
+// memory.  A quad of lanes covers 8 consecutive columns: 32 bytes of the fp32 output, 16 bytes of the 16-bit one.
 template <int BN>
-__device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, const uint32_t (&v)[32], int row, int col0) {
-  if (row >= g.m) return;
-  if (g.vec_ok && col0 + 32 <= g.n) {
-    float f[32];
+__device__ __forceinline__ void epilogue_direct(const GemmArgs& g, float (&acc)[BN / 2], int row0, int col0) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-    if (g.bias != nullptr) {
-      const float4* b4 = reinterpret_cast<const float4*>(g.bias + col0);
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= g.n) continue;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 b = __ldg(b4 + j);
-        f[4 * j + 0] += b.x;
-        f[4 * j + 1] += b.y;
-        f[4 * j + 2] += b.z;
-        f[4 * j + 3] += b.w;
-      }
-    }
-    if (g.act == AB_ACT_GELU_ERF) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 2) gelu_erf_x2(f[j], f[j + 1]);
-    }
-    if (g.residual != nullptr) {
-      const float4* r4 = reinterpret_cast<const float4*>(g.residual + static_cast<size_t>(row) * g.ldr + col0);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 r = __ldg(r4 + j);
-        f[4 * j + 0] += r.x;
-        f[4 * j + 1] += r.y;
-        f[4 * j + 2] += r.z;
-        f[4 * j + 3] += r.w;
-      }
-    }
-    if (g.out_f32 != nullptr) {
-      float4* o4 = reinterpret_cast<float4*>(g.out_f32 + static_cast<size_t>(row) * g.ld_f32 + col0);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) o4[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-    }
-    if (g.out_bf16 != nullptr) {
-      uint4* o4 = reinterpret_cast<uint4*>(g.out_bf16 + static_cast<size_t>(row) * g.ld_bf16 + col0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint4 p;
-        if (g.out_half) {
-          p.x = pack_f16x2(f[8 * j + 0], f[8 * j + 1]);
-          p.y = pack_f16x2(f[8 * j + 2], f[8 * j + 3]);
-          p.z = pack_f16x2(f[8 * j + 4], f[8 * j + 5]);
-          p.w = pack_f16x2(f[8 * j + 6], f[8 * j + 7]);
-        } else {
-          p.x = pack_bf16x2(f[8 * j + 0], f[8 * j + 1]);
-          p.y = pack_bf16x2(f[8 * j + 2], f[8 * j + 3]);
-          p.z = pack_bf16x2(f[8 * j + 4], f[8 * j + 5]);
-          p.w = pack_bf16x2(f[8 * j + 6], f[8 * j + 7]);
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      if (row >= g.m) continue;
+      float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+      bias_act2(g, col, x0, x1);
+      if (g.vec_ok && col + 1 < g.n) {
+        if (g.residual != nullptr) {
+          const float2 r = __ldg(reinterpret_cast<const float2*>(g.residual + static_cast<size_t>(row) * g.ldr + col));
+          x0 += r.x;
+          x1 += r.y;
         }
-        o4[j] = p;
-      }
-    }
-  } else {
+        if (g.out_f32 != nullptr)
+          *reinterpret_cast<float2*>(g.out_f32 + static_cast<size_t>(row) * g.ld_f32 + col) = make_float2(x0, x1);
+        if (g.out_bf16 != nullptr)
+          *reinterpret_cast<uint32_t*>(g.out_bf16 + static_cast<size_t>(row) * g.ld_bf16 + col) =
+              g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
+      } else {
+        const float x[2] = {x0, x1};
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      int col = col0 + j;
-      if (col >= g.n) continue;
-      float x = __uint_as_float(v[j]);
-      if (g.bias != nullptr) x += __ldg(g.bias + col);
-      if (g.act == AB_ACT_GELU_ERF) x = gelu_erf(x);
-      if (g.residual != nullptr) x += __ldg(g.residual + static_cast<size_t>(row) * g.ldr + col);
-      if (g.out_f32 != nullptr) g.out_f32[static_cast<size_t>(row) * g.ld_f32 + col] = x;
-      if (g.out_bf16 != nullptr) g.out_bf16[static_cast<size_t>(row) * g.ld_bf16 + col] = to16(x, g.out_half);
+        for (int e = 0; e < 2; ++e) {
+          if (col + e >= g.n) continue;
+          float v = x[e];
+          if (g.residual != nullptr) v += __ldg(g.residual + static_cast<size_t>(row) * g.ldr + col + e);
+          if (g.out_f32 != nullptr) g.out_f32[static_cast<size_t>(row) * g.ld_f32 + col + e] = v;
+          if (g.out_bf16 != nullptr) g.out_bf16[static_cast<size_t>(row) * g.ld_bf16 + col + e] = to16(v, g.out_half);
+        }
+      }
     }
   }
 }
 
-// Bias / activation on 32 accumulator columns of one row, converted to 16 bit and written as four 16-byte
-// chunks into the warp's staging box (row = lane, 128 bytes per row, 128B swizzle: chunk ^= row & 7, the
-// layout a CU_TENSOR_MAP_SWIZZLE_128B store expects).  `chunk0` = 0 or 4 (first / second 32 columns).
+// 16-bit-only epilogue: per 64-column box, bias / activation on the registers, 16-bit pairs into this warp's staging
+// box (16 rows x 128 bytes, 128B swizzle: chunk ^= row & 7, the layout a CU_TENSOR_MAP_SWIZZLE_128B store expects;
+// the 8 rows x 4 lanes of one store instruction hit 32 different banks), then one asynchronous TMA store: full
+// 128-byte rows, M / N tails clipped by the tensor map.  Rows that a neighbouring GPU needs are copied out of the
+// staging box into its halo slot, 16 bytes per lane.
 template <int BN>
-__device__ __forceinline__ void epilogue_stage_half(const GemmArgs& g, const uint32_t (&v)[32], int col0,
-                                                    uint32_t stage_row, int lane, int chunk0,
-                                                    uint16_t* peer_row = nullptr) {
-  float f[32];
+__device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmap_out, float (&acc)[BN / 2],
+                                             uint8_t* stage, int warp_row0, int n0, int lane) {
+  const int r = lane >> 2, t = lane & 3;
+  const uint32_t st0 = smem_u32(stage) + r * 128 + t * 4;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-  if (g.bias != nullptr) {
-    if (col0 + 32 <= g.n) {
-      const float4* b4 = reinterpret_cast<const float4*>(g.bias + col0);
+  for (int c = 0; c < BN / 64; ++c) {
+    const int colb = n0 + 64 * c;
+    if (colb >= g.n) continue;  // warp-uniform
+    if (lane == 0) tma_store_wait_read<0>();  // the previous box of this warp has left the staging buffer
+    __syncwarp();
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 b = __ldg(b4 + j);
-        f32x2_unpack(f32x2_add(f32x2_pack(f[4 * j + 0], f[4 * j + 1]), f32x2_pack(b.x, b.y)), f[4 * j + 0], f[4 * j + 1]);
-        f32x2_unpack(f32x2_add(f32x2_pack(f[4 * j + 2], f[4 * j + 3]), f32x2_pack(b.z, b.w)), f[4 * j + 2], f[4 * j + 3]);
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = 8 * c + jj;
+      const int col = colb + 8 * jj + 2 * t;
+      float x0 = acc[4 * j], x1 = acc[4 * j + 1], y0 = acc[4 * j + 2], y1 = acc[4 * j + 3];
+      bias_act2(g, col, x0, x1);
+      bias_act2(g, col, y0, y1);
+      const uint32_t off = static_cast<uint32_t>((jj ^ (r & 7)) << 4);
+      const uint32_t lo = g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
+      const uint32_t hi = g.out_half ? pack_f16x2(y0, y1) : pack_bf16x2(y0, y1);
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + off), "r"(lo) : "memory");
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + 8 * 128 + off), "r"(hi) : "memory");
+    }
+    if (g.peer.n_ranges > 0) {
+      __syncwarp();
+      bool any = false;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int lr = 4 * i + (lane >> 3), chunk = lane & 7;
+        uint16_t* const dst = peer_row_ptr(g, warp_row0 + lr, colb);
+        if (dst != nullptr) {
+          any = true;
+          *reinterpret_cast<uint4*>(dst + chunk * 8) =
+              *reinterpret_cast<const uint4*>(stage + lr * 128 + ((chunk ^ (lr & 7)) << 4));
+        }
       }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (col0 + j < g.n) f[j] += __ldg(g.bias + col0 + j);
+      if (__any_sync(0xffffffffu, any)) peer_box_done(g, lane);
     }
-  }
-  if (g.act == AB_ACT_GELU_ERF) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 2) gelu_erf_x2(f[j], f[j + 1]);
-  }
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    uint32_t p0, p1, p2, p3;
-    if (g.out_half) {
-      p0 = pack_f16x2(f[8 * j + 0], f[8 * j + 1]);
-      p1 = pack_f16x2(f[8 * j + 2], f[8 * j + 3]);
-      p2 = pack_f16x2(f[8 * j + 4], f[8 * j + 5]);
-      p3 = pack_f16x2(f[8 * j + 6], f[8 * j + 7]);
-    } else {
-      p0 = pack_bf16x2(f[8 * j + 0], f[8 * j + 1]);
-      p1 = pack_bf16x2(f[8 * j + 2], f[8 * j + 3]);
-      p2 = pack_bf16x2(f[8 * j + 4], f[8 * j + 5]);
-      p3 = pack_bf16x2(f[8 * j + 6], f[8 * j + 7]);
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0 && warp_row0 < g.m) {
+      tma_store_2d(tmap_out, stage, colb, warp_row0);
+      tma_store_commit();
     }
-    const uint32_t addr = stage_row + (((chunk0 + j) ^ (lane & 7)) << 4);
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(p0), "r"(p1), "r"(p2), "r"(p3) : "memory");
-    if (peer_row != nullptr)  // the same 16 bytes straight into the neighbour's halo slot (this lane's row)
-      *reinterpret_cast<uint4*>(peer_row + (chunk0 + j) * 8) = make_uint4(p0, p1, p2, p3);
   }
 }
 
@@ -233,42 +223,30 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   uint8_t* smem_stage_out = smem + Cfg::kStages * Cfg::kStageBytes;  // 1024-byte aligned (stages are)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
   const int warp = threadIdx.x >> 5;  // warp-uniform
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_w);
     if (g.tma_out) prefetch_tmap(&tmap_out);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full_bar[s], 1);
-      mbar_init(&tmem_empty_bar[s], kNumEpiWarps);
+      mbar_init(&empty_bar[s], kMathWarps);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_n = (g.n + BN - 1) / BN;
   const int num_m = (g.m + kBlockM - 1) / kBlockM;
   const int num_tiles = num_m * num_n;
   const int num_kb = (g.k + kBlockK - 1) / kBlockK;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       // ===== TMA producer =====
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -284,97 +262,43 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc = umma_idesc_f16kind_f32(kBlockM, BN, kHalfIn);
-      uint32_t it = 0, tc = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tc) {
-        const uint32_t as = tc & 1u;
-        const uint32_t aph = (tc >> 1) & 1u;
-        mbar_wait(&tmem_empty_bar[as], aph ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const uint32_t s = it % Cfg::kStages;
-          const uint32_t ph = (it / Cfg::kStages) & 1u;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA);
-          const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            const uint64_t da = umma_desc_k_sw128(a_addr + k * kUmmaK * 2);
-            const uint64_t db = umma_desc_k_sw128(b_addr + k * kUmmaK * 2);
-            umma_bf16_ss(tmem_d, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);                           // smem slot free once these MMAs retire
-          if (kb == num_kb - 1) umma_commit(&tmem_full_bar[as]);  // accumulator ready for the epilogue
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue =====
-    const int q = warp & 3;              // TMEM lane quadrant this warp may access
-    const int half = (warp - 4) >> 2;    // column half of the tile
-    uint32_t tc = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tc) {
+  } else {
+    // ===== math warpgroups: rows [64 wg, 64 wg + 64) of the tile =====
+    reg_alloc<232>();
+    const int wg = (warp >> 2) - 1;
+    const int warp_row = wg * 64 + (warp & 3) * kBoxRows;  // first of this warp's 16 accumulator rows inside the tile
+    uint8_t* const stage = smem_stage_out + (warp - 4) * (kBoxRows * 128);
+    float acc[BN / 2];
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m0 = (tile / num_n) * kBlockM;
       const int n0 = (tile % num_n) * BN;
-      const uint32_t as = tc & 1u;
-      const uint32_t aph = (tc >> 1) & 1u;
-      mbar_wait(&tmem_full_bar[as], aph);
-      tc_fence_after_sync();
-      const int row = m0 + q * 32 + lane;
-      if (g.tma_out) {
-        // 16-bit output: TMEM -> registers -> 128B-swizzled smem box {64 cols x 32 rows} -> TMA store.
-        // Stores are full 128-byte rows and asynchronous; M / N tails are clipped by the tensor map.
-        uint8_t* stage = smem_stage_out + (warp - 4) * 4096;
-        const uint32_t stage_row = smem_u32(stage) + lane * 128;
-#pragma unroll 1
-        for (int c = half * 64; c < BN; c += 128) {  // 64-column boxes, interleaved between the two warp sets
-          if (n0 + c >= g.n) break;                   // warp-uniform
-          uint32_t v0[32], v1[32];
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + c;
-          tmem_ld_32x32b_x32(taddr, v0);
-          tmem_ld_32x32b_x32(taddr + 32, v1);
-          tmem_ld_wait();
-          if (lane == 0) tma_store_wait_read<0>();  // previous box of this warp has left the staging buffer
-          __syncwarp();
-          uint16_t* const peer_row = peer_row_ptr(g, row, n0 + c);
-          const bool peer_box = g.peer.n_ranges > 0 && __any_sync(0xffffffffu, peer_row != nullptr);
-          epilogue_stage_half<BN>(g, v0, n0 + c, stage_row, lane, 0, peer_row);
-          epilogue_stage_half<BN>(g, v1, n0 + c + 32, stage_row, lane, 4, peer_row);
-          if (peer_box) peer_box_done(g, lane);
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&tmap_out, stage, n0 + c, m0 + q * 32);
-            tma_store_commit();
-          }
+      int prev_s = -1;
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const uint32_t s = it % Cfg::kStages;
+        mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1u);
+        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + wg * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
+        wgmma_fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+          wgmma_ss<BN, kHalfIn>(acc, wgmma_desc_sw128(a_addr + k * kWgmmaK * 2), wgmma_desc_sw128(b_addr + k * kWgmmaK * 2),
+                                (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (prev_s >= 0) {
+          wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand its shared memory back to the producer
+          if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
         }
-      } else {
-#pragma unroll 1
-        for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + c, v);
-          tmem_ld_wait();
-          epilogue_chunk<BN>(g, v, row, n0 + c);
-        }
+        prev_s = static_cast<int>(s);
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[as]);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
+      if (g.tma_out) epilogue_tma<BN>(g, &tmap_out, acc, stage, m0 + warp_row, n0, lane);
+      else epilogue_direct<BN>(g, acc, m0 + warp_row + (lane >> 2), n0 + 2 * (lane & 3));
     }
-  }
-
-  if (warp >= 4 && g.tma_out && lane == 0) tma_store_wait_all<0>();  // smem must outlive the bulk stores
-  __syncwarp();
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+    if (g.tma_out && lane == 0) tma_store_wait_all<0>();  // smem must outlive the bulk stores
   }
 }
 
@@ -388,7 +312,7 @@ static int launch_gemm(const AbGemm* p, const GemmArgs& args, cudaStream_t strea
   if (rc != AB_OK) return rc;
   CUtensorMap tout = ta;  // placeholder when unused
   if (args.tma_out) {
-    rc = make_tmap_16bit_2d(&tout, p->out_bf16, p->m, p->n, p->ld_bf16, 32, 64, args.out_half != 0);
+    rc = make_tmap_16bit_2d(&tout, p->out_bf16, p->m, p->n, p->ld_bf16, kBoxRows, 64, args.out_half != 0);
     if (rc != AB_OK) return rc;
   }
   static bool attr_set = false;
@@ -407,504 +331,6 @@ static int launch_gemm(const AbGemm* p, const GemmArgs& args, cudaStream_t strea
   AB_COUNT_LAUNCH(1);
   AB_CHECK_LAUNCH("ab_gemm_bf16");
   return AB_OK;
-}
-
-
-// ================================================================================================
-// CTA-pair variant (cta_group::2): one 256 x 256 output tile per cluster of two CTAs.
-//
-// Each CTA stages its own 128 rows of A and HALF of the W tile (128 of the 256 N rows); the leader CTA
-// issues tcgen05.mma.cta_group::2 (M = 256) which reads both CTAs' shared memory and writes 128 accumulator
-// rows into each CTA's TMEM.  Per SM this cuts operand traffic per k-step from (128 + 256) to (128 + 128)
-// rows, i.e. shared-memory port load (tensor reads + TMA writes) from 192 to 128 B/clk — the single-CTA
-// kernel is capped at ~65 % tensor-pipe utilisation by that port (profiles/r01_*).
-//   full barrier   : leader's, count 2 (leader arrive.expect_tx for all four loads + peer remote arrive)
-//   empty barrier  : per CTA, signalled by a multicast tcgen05.commit from the leader
-//   tmem full      : per CTA, multicast commit;  tmem empty: leader's, 2 x 8 epilogue-warp arrivals
-// ================================================================================================
-template <bool kHalfIn>
-struct Gemm2Cfg {
-  static constexpr int BN = 256;                       // cluster tile N
-  static constexpr int kLoadN = 128;                   // W rows staged per CTA
-  static constexpr int kStageBytesA = kBlockM * kBlockK * 2;
-  static constexpr int kStageBytesB = kLoadN * kBlockK * 2;
-  static constexpr int kStageBytes = kStageBytesA + kStageBytesB;  // 32 KB
-  static constexpr int kStages = 6;
-  static constexpr uint32_t kTmemCols = 2 * BN;
-  static constexpr int kBarrierBytes = 256;
-  static constexpr int kStagingBytes = kNumEpiWarps * 4096;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBarrierBytes + 1024;
-};
-
-template <bool kHalfIn>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kNumThreads, 1)
-gemm2_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
-                     const __grid_constant__ CUtensorMap tmap_out, const GemmArgs g) {
-  using Cfg = Gemm2Cfg<kHalfIn>;
-  constexpr int BN = Cfg::BN;
-  extern __shared__ uint8_t smem_raw[];
-  // Both CTAs must carve shared memory identically (descriptors / barrier offsets are shared).
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + Cfg::kStages * Cfg::kStageBytesA;
-  uint8_t* smem_stage_out = smem + Cfg::kStages * Cfg::kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  cluster_sync_all();  // both CTAs resident before the pair-wide TMEM allocation
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_w);
-    if (g.tma_out) prefetch_tmap(&tmap_out);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 2);   // used in the leader only
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full_bar[s], 1);
-      mbar_init(&tmem_empty_bar[s], 2 * kNumEpiWarps);  // used in the leader only
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc_pair<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before_sync();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int num_n = (g.n + BN - 1) / BN;
-  const int num_mp = (g.m + 2 * kBlockM - 1) / (2 * kBlockM);  // 256-row tile pairs
-  const int num_tiles = num_mp * num_n;
-  const int num_kb = (g.k + kBlockK - 1) / kBlockK;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (both CTAs) =====
-      uint32_t it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        const int m0 = (tile / num_n) * (2 * kBlockM) + rank * kBlockM;
-        const int n0 = (tile % num_n) * BN + rank * Cfg::kLoadN;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const uint32_t s = it % Cfg::kStages;
-          const uint32_t ph = (it / Cfg::kStages) & 1u;
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          tma_load_2d_pair(smem_a + s * Cfg::kStageBytesA, &tmap_a, &full_bar[s], kb * kBlockK, m0);
-          tma_load_2d_pair(smem_b + s * Cfg::kStageBytesB, &tmap_w, &full_bar[s], kb * kBlockK, n0);
-          if (leader) mbar_arrive_expect_tx(&full_bar[s], 2 * Cfg::kStageBytes);
-          else mbar_arrive_remote(&full_bar[s], 0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ===== MMA issuer (leader CTA only) =====
-      constexpr uint32_t idesc = umma_idesc_f16kind_f32(2 * kBlockM, BN, kHalfIn);
-      uint32_t it = 0, tc = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tc) {
-        const uint32_t as = tc & 1u;
-        const uint32_t aph = (tc >> 1) & 1u;
-        mbar_wait(&tmem_empty_bar[as], aph ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const uint32_t s = it % Cfg::kStages;
-          const uint32_t ph = (it / Cfg::kStages) & 1u;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA);
-          const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            const uint64_t da = umma_desc_k_sw128(a_addr + k * kUmmaK * 2);
-            const uint64_t db = umma_desc_k_sw128(b_addr + k * kUmmaK * 2);
-            umma_bf16_ss_pair(tmem_d, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_pair(&empty_bar[s]);
-          if (kb == num_kb - 1) umma_commit_pair(&tmem_full_bar[as]);
-        }
-      }
-      // Let the last remote arrivals land on our barriers before the CTA may exit.
-      if (tc > 0) {
-        const uint32_t last = tc - 1;
-        mbar_wait(&tmem_empty_bar[last & 1u], (last >> 1) & 1u);
-        if (tc > 1) {
-          const uint32_t prev = tc - 2;
-          mbar_wait(&tmem_empty_bar[prev & 1u], (prev >> 1) & 1u);
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue (each CTA: its own 128 accumulator rows) =====
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
-    uint32_t tc = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tc) {
-      const int m0 = (tile / num_n) * (2 * kBlockM) + rank * kBlockM;
-      const int n0 = (tile % num_n) * BN;
-      const uint32_t as = tc & 1u;
-      const uint32_t aph = (tc >> 1) & 1u;
-      mbar_wait(&tmem_full_bar[as], aph);
-      tc_fence_after_sync();
-      const int row = m0 + q * 32 + lane;
-      if (g.tma_out) {
-        uint8_t* stage = smem_stage_out + (warp - 4) * 4096;
-        const uint32_t stage_row = smem_u32(stage) + lane * 128;
-#pragma unroll 1
-        for (int c = half * 64; c < BN; c += 128) {
-          if (n0 + c >= g.n) break;
-          uint32_t v0[32], v1[32];
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + c;
-          tmem_ld_32x32b_x32(taddr, v0);
-          tmem_ld_32x32b_x32(taddr + 32, v1);
-          tmem_ld_wait();
-          if (lane == 0) tma_store_wait_read<0>();
-          __syncwarp();
-          uint16_t* const peer_row = peer_row_ptr(g, row, n0 + c);
-          const bool peer_box = g.peer.n_ranges > 0 && __any_sync(0xffffffffu, peer_row != nullptr);
-          epilogue_stage_half<BN>(g, v0, n0 + c, stage_row, lane, 0, peer_row);
-          epilogue_stage_half<BN>(g, v1, n0 + c + 32, stage_row, lane, 4, peer_row);
-          if (peer_box) peer_box_done(g, lane);
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0 && m0 + q * 32 < g.m) {
-            tma_store_2d(&tmap_out, stage, n0 + c, m0 + q * 32);
-            tma_store_commit();
-          }
-        }
-      } else {
-#pragma unroll 1
-        for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN + c, v);
-          tmem_ld_wait();
-          epilogue_chunk<BN>(g, v, row, n0 + c);
-        }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&tmem_empty_bar[as], 0);  // the leader's barrier collects both CTAs
-    }
-  }
-
-  if (warp >= 4 && g.tma_out && lane == 0) tma_store_wait_all<0>();
-  __syncwarp();
-  tc_fence_before_sync();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
-  }
-}
-
-template <bool kHalfIn>
-static int launch_gemm2(const AbGemm* p, const GemmArgs& args, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<kHalfIn>;
-  CUtensorMap ta, tw;
-  int rc = make_tmap_16bit_2d(&ta, p->a, p->m, p->k, p->lda, kBlockM, kBlockK, kHalfIn);
-  if (rc != AB_OK) return rc;
-  rc = make_tmap_16bit_2d(&tw, p->w, p->n, p->k, p->ldw, Cfg::kLoadN, kBlockK, kHalfIn);
-  if (rc != AB_OK) return rc;
-  CUtensorMap tout = ta;
-  if (args.tma_out) {
-    rc = make_tmap_16bit_2d(&tout, p->out_bf16, p->m, p->n, p->ld_bf16, 32, 64, args.out_half != 0);
-    if (rc != AB_OK) return rc;
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm2_bf16_tn_kernel<kHalfIn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes);
-    if (e != cudaSuccess) {
-      set_error("ab_gemm_bf16: cudaFuncSetAttribute(pair, smem=%d) failed: %s", Cfg::kSmemBytes,
-                cudaGetErrorString(e));
-      return AB_ERR_CUDA;
-    }
-    attr_set = true;
-  }
-  const long long tiles = ceil_div_ll(p->m, 2 * kBlockM) * ceil_div_ll(p->n, Cfg::BN);
-  const long long max_clusters = sm_count() / 2;
-  const int clusters = static_cast<int>(tiles < max_clusters ? tiles : max_clusters);
-  gemm2_bf16_tn_kernel<kHalfIn><<<2 * clusters, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
-  AB_COUNT_LAUNCH(1);
-  AB_CHECK_LAUNCH("ab_gemm_bf16(pair)");
-  return AB_OK;
-}
-
-
-// ================================================================================================
-// Wide CTA-pair variant: one 512 x 256 output tile per cluster of two CTAs (256 x 256 per CTA).
-//
-// ncu on the 256 x 256 pair kernel shows the large-K GEMMs of this model are bound by L2 -> SM delivery, not by
-// the tensor pipe: l1tex__m_xbar2l1tex_read_bytes / duration = 10.8 TB/s = 6.6 KB/clk chip-wide, the LTS cap
-// (profiles/r01_ncu_full_summaries.md, r01j; cuBLAS' nvjet 256x256-per-CTA kernel moves 0.75x the bytes).  Staging
-// 256 rows of A per CTA against the same half W tile cuts operand bytes per flop by 25 %:
-//   per k-block and CTA: A 2 x (128 x 64) + W 128 x 64 = 48 KB for two M=256 MMAs (was 32 KB for one).
-// The two accumulators (one per 128-row half, 256 fp32 columns each) fill all 512 TMEM columns, so there is no
-// spare accumulator to double-buffer with.  Instead the MMA issuer staggers the two accumulators at the tile
-// boundaries only: acc 0 takes the last kLag k-blocks of a tile before acc 1 does, so acc 0 finishes first and the
-// epilogue warps drain it while the tensor pipe finishes acc 1; the next tile starts with kLag k-blocks on acc 0,
-// which cover the drain of acc 1.  In between both advance in lockstep so that all 4 stages (192 KB) stay in
-// flight — a permanently lagging acc 1 (tried first) pins kLag stages and starves the L2-latency-bound loads.
-// Used for plain (no activation) epilogues with K >= 1024, where a drain is short against the main loop.
-// ================================================================================================
-template <bool kHalfIn>
-struct Gemm2wCfg {
-  static constexpr int BN = 256;
-  static constexpr int kLoadN = 128;
-  static constexpr int kSubA = kBlockM * kBlockK * 2;         // one 128-row half of A: 16 KB
-  static constexpr int kStageBytesA = 2 * kSubA;
-  static constexpr int kStageBytesB = kLoadN * kBlockK * 2;
-  static constexpr int kStageBytes = kStageBytesA + kStageBytesB;  // 48 KB
-  static constexpr int kStages = 4;
-  static constexpr int kLag = 2;  // k-blocks accumulator 0 leads by at the tile boundaries
-  static constexpr uint32_t kTmemCols = 2 * BN;
-  static constexpr int kBarrierBytes = 256;
-  static constexpr int kStagingBytes = kNumEpiWarps * 4096;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBarrierBytes + 1024;
-};
-
-template <bool kHalfIn>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kNumThreads, 1)
-gemm2w_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
-                      const __grid_constant__ CUtensorMap tmap_out, const GemmArgs g) {
-  using Cfg = Gemm2wCfg<kHalfIn>;
-  constexpr int BN = Cfg::BN;
-  constexpr int kTileM = 4 * kBlockM;  // 512 rows per cluster tile
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + Cfg::kStages * Cfg::kStageBytesA;
-  uint8_t* smem_stage_out = smem + Cfg::kStages * Cfg::kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;  // [h]: accumulator h holds a finished tile
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [h]: accumulator h has been read out (leader's)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  cluster_sync_all();
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_w);
-    if (g.tma_out) prefetch_tmap(&tmap_out);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 2);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int h = 0; h < 2; ++h) {
-      mbar_init(&tmem_full_bar[h], 1);
-      mbar_init(&tmem_empty_bar[h], 2 * kNumEpiWarps);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc_pair<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before_sync();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int num_n = (g.n + BN - 1) / BN;
-  const int num_mt = (g.m + kTileM - 1) / kTileM;
-  const int num_tiles = num_mt * num_n;
-  const int num_kb = (g.k + kBlockK - 1) / kBlockK;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (both CTAs): rows [m0, m0 + 256) of A as two 128-row boxes, 128 rows of W =====
-      uint32_t it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        const int m0 = (tile / num_n) * kTileM + rank * (2 * kBlockM);
-        const int n0 = (tile % num_n) * BN + rank * Cfg::kLoadN;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const uint32_t s = it % Cfg::kStages;
-          const uint32_t ph = (it / Cfg::kStages) & 1u;
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          uint8_t* sa = smem_a + s * Cfg::kStageBytesA;
-          tma_load_2d_pair(sa, &tmap_a, &full_bar[s], kb * kBlockK, m0);
-          tma_load_2d_pair(sa + Cfg::kSubA, &tmap_a, &full_bar[s], kb * kBlockK, m0 + kBlockM);
-          tma_load_2d_pair(smem_b + s * Cfg::kStageBytesB, &tmap_w, &full_bar[s], kb * kBlockK, n0);
-          if (leader) mbar_arrive_expect_tx(&full_bar[s], 2 * Cfg::kStageBytes);
-          else mbar_arrive_remote(&full_bar[s], 0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ===== MMA issuer (leader CTA only) =====
-      // Issue order per tile: the two accumulators advance in lockstep (all stages stay in flight), except that
-      // accumulator 0 takes the first and the last kLag k-blocks of the tile ahead of accumulator 1 — see above.
-      constexpr uint32_t idesc = umma_idesc_f16kind_f32(2 * kBlockM, BN, kHalfIn);
-      uint32_t base_it = 0, tc = 0;  // k-blocks consumed before this tile
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tc) {
-        const uint32_t tph = tc & 1u;
-        auto issue = [&](int h, int kb) {
-          const uint32_t it = base_it + kb;
-          const uint32_t s = it % Cfg::kStages;
-          if (kb == 0) mbar_wait(&tmem_empty_bar[h], tph ^ 1u);
-          if (h == 0) mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1u);  // acc 1 always follows acc 0 on a stage
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA + h * Cfg::kSubA);
-          const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k)
-            umma_bf16_ss_pair(tmem_base + h * BN, umma_desc_k_sw128(a_addr + k * kUmmaK * 2),
-                              umma_desc_k_sw128(b_addr + k * kUmmaK * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-          if (h == 1) umma_commit_pair(&empty_bar[s]);  // both halves of the stage are consumed
-          if (kb == num_kb - 1) umma_commit_pair(&tmem_full_bar[h]);
-        };
-        constexpr int X = Cfg::kLag;
-        if (X > 0 && num_kb >= 2 * X) {
-          for (int kb = 0; kb < X; ++kb) issue(0, kb);
-          for (int kb = 0; kb < X; ++kb) issue(1, kb);
-          for (int kb = X; kb < num_kb - X; ++kb) {
-            issue(0, kb);
-            issue(1, kb);
-          }
-          for (int kb = num_kb - X; kb < num_kb; ++kb) issue(0, kb);
-          for (int kb = num_kb - X; kb < num_kb; ++kb) issue(1, kb);
-        } else {
-          for (int kb = 0; kb < num_kb; ++kb) {
-            issue(0, kb);
-            issue(1, kb);
-          }
-        }
-        base_it += num_kb;
-      }
-      // Let the last remote arrivals land on our barriers before the CTA may exit.
-      if (tc > 0) {
-        const uint32_t last = tc - 1;
-        mbar_wait(&tmem_empty_bar[0], last & 1u);
-        mbar_wait(&tmem_empty_bar[1], last & 1u);
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: accumulator 0 (rows +0..127 of this CTA's 256), then accumulator 1 (rows +128..255) =====
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
-    uint32_t tc = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tc) {
-      const int n0 = (tile % num_n) * BN;
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        const int m0 = (tile / num_n) * kTileM + rank * (2 * kBlockM) + h * kBlockM;
-        mbar_wait(&tmem_full_bar[h], tc & 1u);
-        tc_fence_after_sync();
-        const int row = m0 + q * 32 + lane;
-        const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + h * BN;
-        if (g.tma_out) {
-          uint8_t* stage = smem_stage_out + (warp - 4) * 4096;
-          const uint32_t stage_row = smem_u32(stage) + lane * 128;
-#pragma unroll 1
-          for (int c = half * 64; c < BN; c += 128) {
-            const bool live = n0 + c < g.n;
-            const bool last = c + 128 >= BN;
-            uint32_t v0[32], v1[32];
-            tmem_ld_32x32b_x32(tacc + c, v0);
-            tmem_ld_32x32b_x32(tacc + c + 32, v1);
-            tmem_ld_wait();
-            if (last) {
-              // everything this warp needs from the accumulator is in registers: hand it back before the math
-              tc_fence_before_sync();
-              __syncwarp();
-              if (lane == 0) mbar_arrive_remote(&tmem_empty_bar[h], 0);
-            }
-            if (!live) continue;
-            if (lane == 0) tma_store_wait_read<0>();
-            __syncwarp();
-            uint16_t* const peer_row = peer_row_ptr(g, row, n0 + c);
-            const bool peer_box = g.peer.n_ranges > 0 && __any_sync(0xffffffffu, peer_row != nullptr);
-            epilogue_stage_half<BN>(g, v0, n0 + c, stage_row, lane, 0, peer_row);
-            epilogue_stage_half<BN>(g, v1, n0 + c + 32, stage_row, lane, 4, peer_row);
-            if (peer_box) peer_box_done(g, lane);
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0 && m0 + q * 32 < g.m) {
-              tma_store_2d(&tmap_out, stage, n0 + c, m0 + q * 32);
-              tma_store_commit();
-            }
-          }
-        } else {
-#pragma unroll 1
-          for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(tacc + c, v);
-            tmem_ld_wait();
-            epilogue_chunk<BN>(g, v, row, n0 + c);
-          }
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_remote(&tmem_empty_bar[h], 0);
-        }
-      }
-    }
-  }
-
-  if (warp >= 4 && g.tma_out && lane == 0) tma_store_wait_all<0>();
-  __syncwarp();
-  tc_fence_before_sync();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
-  }
-}
-
-template <bool kHalfIn>
-static int launch_gemm2w(const AbGemm* p, const GemmArgs& args, cudaStream_t stream) {
-  using Cfg = Gemm2wCfg<kHalfIn>;
-  CUtensorMap ta, tw;
-  int rc = make_tmap_16bit_2d(&ta, p->a, p->m, p->k, p->lda, kBlockM, kBlockK, kHalfIn);
-  if (rc != AB_OK) return rc;
-  rc = make_tmap_16bit_2d(&tw, p->w, p->n, p->k, p->ldw, Cfg::kLoadN, kBlockK, kHalfIn);
-  if (rc != AB_OK) return rc;
-  CUtensorMap tout = ta;
-  if (args.tma_out) {
-    rc = make_tmap_16bit_2d(&tout, p->out_bf16, p->m, p->n, p->ld_bf16, 32, 64, args.out_half != 0);
-    if (rc != AB_OK) return rc;
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm2w_bf16_tn_kernel<kHalfIn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes);
-    if (e != cudaSuccess) {
-      set_error("ab_gemm_bf16: cudaFuncSetAttribute(wide pair, smem=%d) failed: %s", Cfg::kSmemBytes,
-                cudaGetErrorString(e));
-      return AB_ERR_CUDA;
-    }
-    attr_set = true;
-  }
-  const long long tiles = ceil_div_ll(p->m, 4 * kBlockM) * ceil_div_ll(p->n, Cfg::BN);
-  const long long max_clusters = sm_count() / 2;
-  const int clusters = static_cast<int>(tiles < max_clusters ? tiles : max_clusters);
-  gemm2w_bf16_tn_kernel<kHalfIn><<<2 * clusters, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
-  AB_COUNT_LAUNCH(1);
-  AB_CHECK_LAUNCH("ab_gemm_bf16(wide pair)");
-  return AB_OK;
-}
-
-// Wave efficiency of a persistent launch: useful tiles / (waves x resident clusters).
-static double wave_efficiency(long long tiles, long long slots) {
-  const long long waves = (tiles + slots - 1) / slots;
-  return static_cast<double>(tiles) / static_cast<double>(waves * slots);
 }
 
 }  // namespace ab
@@ -980,7 +406,7 @@ extern "C" int ab_gemm_bf16(const AbGemm* p, void* stream) {
       }
     }
     AB_CHECK_ARG(pr.n_ranges > 0, "ab_gemm_bf16: peer_push with nothing to send (use ab_halo_push, which still publishes)");
-    // boxes of this launch that carry peer rows: distinct 32-row groups touched by any range x 64-column boxes sent
+    // boxes of this launch that carry peer rows: distinct 16-row groups touched by any range x 64-column boxes sent
     int groups = 0, last_group = -1;
     for (int pass = 0; pass < 1; ++pass) {
       // ranges are emitted in increasing row order per level, and levels increase: a sweep over sorted begins suffices
@@ -994,8 +420,8 @@ extern "C" int ab_gemm_bf16(const AbGemm* p, void* stream) {
         }
       for (int k = 0; k < pr.n_ranges; ++k) {
         const int i = order[k];
-        int g0 = pr.row_begin[i] / 32;
-        const int g1 = (pr.row_end[i] - 1) / 32;
+        int g0 = pr.row_begin[i] / kBoxRows;
+        const int g1 = (pr.row_end[i] - 1) / kBoxRows;
         if (g0 <= last_group) g0 = last_group + 1;
         if (g1 >= g0) groups += g1 - g0 + 1;
         if (g1 > last_group) last_group = g1;
@@ -1004,25 +430,6 @@ extern "C" int ab_gemm_bf16(const AbGemm* p, void* stream) {
     pr.expected = groups * ((p->n - pr.col_from + 63) / 64);
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  // Large problems run on CTA pairs (cta_group::2); small or narrow ones on the single-CTA kernel.
-  static const bool pair_disabled = getenv("AB_GEMM_NO_PAIR") != nullptr;
-  if (!pair_disabled && p->n >= 256 && p->m >= 1024) {
-    // 512 x 256 tiles (25 % fewer operand bytes through the L2 -> SM path) pay off when the main loop is long
-    // against the accumulator drain (K >= 2048, plain epilogue) and the coarser tiles do not cost a wave:
-    // measured -5 % (259200 x 512 x 2048) and -9 % (64800 x 1024 x 4096), neutral at K = 1024
-    // (profiles/r01_kernel_probes.md).  AB_GEMM_WIDE: 0 = never, 2 = whenever K >= 1024 (tests).
-    const char* wide_env = getenv("AB_GEMM_WIDE");  // read per call so that tests can flip it
-    const int wide_mode = wide_env ? atoi(wide_env) : 1;
-    bool wide = false;
-    if (wide_mode > 0 && p->k >= 1024) {
-      const long long slots = sm_count() / 2;
-      const double eff_w = wave_efficiency(ceil_div_ll(p->m, 4 * kBlockM) * ceil_div_ll(p->n, 256), slots);
-      const double eff_2 = wave_efficiency(ceil_div_ll(p->m, 2 * kBlockM) * ceil_div_ll(p->n, 256), slots);
-      wide = wide_mode >= 2 || (p->act == AB_ACT_NONE && p->k >= 2048 && eff_w * 1.02 >= eff_2);
-    }
-    if (wide) return p->in_dtype == AB_DT_F16 ? launch_gemm2w<true>(p, a, s) : launch_gemm2w<false>(p, a, s);
-    return p->in_dtype == AB_DT_F16 ? launch_gemm2<true>(p, a, s) : launch_gemm2<false>(p, a, s);
-  }
   if (p->in_dtype == AB_DT_F16) {
     if (p->n > 128) return launch_gemm<256, true>(p, a, s);
     if (p->n > 64) return launch_gemm<128, true>(p, a, s);

@@ -7,50 +7,39 @@
 // per model time step).  Unfused, the projection writes y in 16 bit and a row kernel reads y + the fp32 stream back and
 // writes the stream + its 16-bit copy: 14 B of HBM traffic per element; fused it is 10 B and one launch less.
 //
-// LayerNorm needs whole rows, so a cluster owns whole rows: N = D = 512 * P columns, P CTA PAIRS per cluster.
-//   * every pair runs the cta_group::2 pipeline of gemm.cu on ITS 512 columns: M = 256 rows per cluster tile (128 per
-//     CTA), two accumulators of 256 fp32 columns = all 512 TMEM columns of both SMs (no accumulator double buffering:
-//     the epilogue is HBM-bound, the next tile's operands are prefetched under it);
-//   * epilogue, 16 warps, one thread per row and 128-column group (warp w: TMEM lane quadrant w & 3, group (w - 4) >> 2);
-//     an otherwise idle warp prefetches the NEXT tile's residual rows into L2 (cp.async.bulk.prefetch) under the
-//     current tile's main loop, so the epilogue's reads are L2 hits:
-//       pass 1  sum(y), sum(y^2) -> mean, rstd   (partials of the four warps that share a row meet in shared memory;
-//                                                 P = 2: + one DSMEM exchange with the CTA holding the other columns)
-//       pass 2  residual + (y - mean) * rstd * scale + shift -> fp32 stream (may alias the residual) + 16-bit copy
-//     two reads of the accumulator out of TMEM (16 TB/s aggregate) instead of one trip through HBM.  Pass 2 turns
-//     the "thread = row" TMEM layout into coalesced global accesses through a 2 KB per-warp shared-memory tile
-//     (32 rows x 16 columns, XOR-swizzled, conflict-free both ways): four lanes read one row's 64 bytes of the
-//     residual, add, and write 64 bytes of the fp32 stream / 32 bytes of the 16-bit copy.  (First version: every
-//     thread streamed its own row with 16-byte accesses — 32 cache lines per warp instruction — and reached 1.2 - 2.9
-//     TB/s; profiles/r02_kernel_probes.md.)
-//   * P = 2 (D = 1024): CTA r exchanges its per-row partial sums with CTA r ^ 2 (same rows, other 512 columns) through
-//     distributed shared memory: remote store + remote mbarrier arrive (release.cluster) / acquire.cluster wait.
+// LayerNorm needs whole rows, so a CLUSTER owns whole rows: N = D = 256 * C columns, C = 2 or 4 CTAs per cluster, every
+// CTA running the wgmma pipeline of gemm.cu on ITS 256 columns of the cluster's 128 rows (two math warpgroups x 64 rows,
+// the 64 x 256 fp32 accumulator in registers).  Epilogue, all on the registers:
+//   1. y = acc + bias; sum(y), sum(y^2) over the thread's 2 x 64 values, reduced over the quad of lanes that shares a row;
+//   2. every CTA stores its per-row partial sums into the other CTAs' shared memory (st.shared::cluster) and arrives on
+//      their mbarrier (release.cluster); after the acquire every CTA holds the statistics of the whole row.  The slots
+//      are double-buffered by tile parity: a CTA can run at most one tile ahead of a neighbour that has not read yet;
+//   3. residual + (y - mean) * rstd * scale + shift -> fp32 stream (may alias the residual) + 16-bit copy.  A quad of
+//      lanes covers 8 consecutive columns: 32-byte sectors of the fp32 stream, 16 bytes of the 16-bit copy.
+// The accumulator is read once and never leaves the registers.
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace ab {
 namespace gln {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
-constexpr int kUmmaK = 16;
-constexpr int kHalfN = 256;          // one accumulator / one MMA N
-constexpr int kPairN = 2 * kHalfN;   // columns per CTA pair
-constexpr int kLoadN = 128;          // W rows staged per CTA and accumulator half
-constexpr int kNumEpiWarps = 16;     // four per TMEM lane quadrant: 128 of the pair's 512 columns each
-constexpr int kColsPerWarp = kPairN / 4;
-constexpr int kThreads = 128 + kNumEpiWarps * 32;
+constexpr int kWgmmaK = 16;
+constexpr int kCtaN = 256;           // columns per CTA = one wgmma N
+constexpr int kMaxCluster = 4;
+constexpr int kMathWarps = 8;
+constexpr int kThreads = 128 + kMathWarps * 32;
 constexpr int kStageBytesA = kBlockM * kBlockK * 2;  // 16 KB
-constexpr int kSubB = kLoadN * kBlockK * 2;          // 16 KB
-constexpr int kStageBytes = kStageBytesA + 2 * kSubB;  // 48 KB
-constexpr int kStages = 3;
-constexpr int kOffVec = kStages * kStageBytes;         // bias | scale | shift of this pair's 512 columns (f32)
-constexpr int kVecBytes = 3 * kPairN * 4;
-constexpr int kOffStat = kOffVec + kVecBytes;          // part[4][128] float2 (sum, sum of squares), rem[128] float2
-constexpr int kStatBytes = (4 * 128 * 2 + 128 * 2) * 4;
-constexpr int kOffStage = (kOffStat + kStatBytes + 127) & ~127;  // per epilogue warp: 32 rows x 16 fp32 columns
-constexpr int kStageOutBytes = 32 * 16 * 4;                     // 2 KB
-constexpr int kOffBar = kOffStage + kNumEpiWarps * kStageOutBytes;
+constexpr int kStageBytesB = kCtaN * kBlockK * 2;    // 32 KB
+constexpr int kStageBytes = kStageBytesA + kStageBytesB;
+constexpr int kStages = 4;
+constexpr int kOffVec = kStages * kStageBytes;         // bias | scale | shift of this CTA's 256 columns (f32)
+constexpr int kVecBytes = 3 * kCtaN * 4;
+constexpr int kOffStat = kOffVec + kVecBytes;          // rem[2][kMaxCluster][128] float2 (sum, sum of squares)
+constexpr int kStatBytes = 2 * kMaxCluster * kBlockM * 8;
+constexpr int kOffBar = kOffStat + kStatBytes;
 constexpr int kBarrierBytes = 256;
 constexpr int kSmemBytes = kOffBar + kBarrierBytes + 1024;
 static_assert(kSmemBytes <= 227 * 1024, "shared memory");
@@ -68,18 +57,15 @@ struct Args {
   float eps;
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-// Remote (DSMEM) float store into CTA `cta` of this cluster at the same shared-memory offset as `p`.
-__device__ __forceinline__ void st_remote_f32(float* p, uint32_t cta, float v) {
+// Remote (DSMEM) float2 store into CTA `cta` of this cluster at the same shared-memory offset as `p`.
+__device__ __forceinline__ void st_remote_f32x2(float2* p, uint32_t cta, float2 v) {
   asm volatile(
       "{\n\t"
       ".reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "st.shared::cluster.f32 [ra], %2;\n\t"
+      "st.shared::cluster.v2.f32 [ra], {%2, %3};\n\t"
       "}\n" ::"r"(smem_u32(p)),
-      "r"(cta), "f"(v)
+      "r"(cta), "f"(v.x), "f"(v.y)
       : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_remote_release(uint64_t* bar, uint32_t cta) {
@@ -113,288 +99,197 @@ __device__ __forceinline__ void mbar_wait_acquire_cluster(uint64_t* bar, uint32_
     }
   }
 }
-// tcgen05.commit arriving on the barrier at this offset in both CTAs of MY pair (cluster ranks pair_base, pair_base + 1)
-__device__ __forceinline__ void umma_commit_pair_of(uint64_t* bar, uint32_t pair_base) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3u << pair_base))
-      : "memory");
-}
 
-template <bool kHalfIn, int P>
-__global__ void __cluster_dims__(2 * P, 1, 1) __launch_bounds__(kThreads, 1)
+template <bool kHalfIn, int C>
+__global__ void __cluster_dims__(C, 1, 1) __launch_bounds__(kThreads, 1)
 gemm_ln_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w, const Args g) {
   extern __shared__ uint8_t smem_raw[];
+  // every CTA of the cluster carves shared memory identically: remote stores address the same offsets
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * kStageBytesA;  // per stage: two 16 KB sub-tiles (accumulator halves)
+  uint8_t* smem_b = smem + kStages * kStageBytesA;
   float* s_bias = reinterpret_cast<float*>(smem + kOffVec);
-  float* s_scale = s_bias + kPairN;
-  float* s_shift = s_scale + kPairN;
-  float2* part = reinterpret_cast<float2*>(smem + kOffStat);  // [4][128]: (sum, sum of squares) per column group and row
-  float2* rem = part + 4 * 128;                               // [128]: the partner CTA's row totals (P = 2)
-  uint8_t* stage_out = smem + kOffStage;                      // 8 x 2 KB transpose tiles
+  float* s_scale = s_bias + kCtaN;
+  float* s_shift = s_scale + kCtaN;
+  float2* rem = reinterpret_cast<float2*>(smem + kOffStat);  // [parity][rank][row]: partial (sum, sum of squares)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kOffBar);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full_bar = empty_bar + kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 1;  // leader's
-  uint64_t* stat_bar = tmem_empty_bar + 1;       // P = 2: the partner CTA's four group-0 warps arrive here
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stat_bar + 1);
+  // [tile parity]: the other CTAs' math warps arrive here once their partials are stored.  Two barriers, like the slots:
+  // the next phase of a barrier needs this CTA's own arrivals of the tile in between, so no waiter can be lapped.
+  uint64_t* stat_bar = empty_bar + kStages;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const uint32_t rank = cluster_ctarank();
-  const uint32_t pair = rank >> 1;            // which 512 columns
-  const uint32_t pair_base = rank & ~1u;      // cluster rank of my pair's leader
-  const bool leader = (rank & 1u) == 0;
-  const int n_base = static_cast<int>(pair) * kPairN;
+  const int n_base = static_cast<int>(rank) * kCtaN;
 
-  cluster_sync_all();
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_w);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full_bar[s], 2);   // leader: own arrive.expect_tx + the peer's remote arrive
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kMathWarps);
     }
-    mbar_init(tmem_full_bar, 1);
-    mbar_init(tmem_empty_bar, 2 * kNumEpiWarps);
-    mbar_init(stat_bar, 4);
+    mbar_init(&stat_bar[0], (C - 1) * kMathWarps);
+    mbar_init(&stat_bar[1], (C - 1) * kMathWarps);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc_pair<512>(tmem_slot);
-  // this pair's slice of the per-column vectors
-  for (int i = threadIdx.x; i < kPairN; i += kThreads) {
+  for (int i = threadIdx.x; i < kCtaN; i += kThreads) {
     s_bias[i] = g.bias != nullptr ? __ldg(g.bias + n_base + i) : 0.f;
     s_scale[i] = g.scale != nullptr ? __ldg(g.scale + n_base + i) : 1.f;
     s_shift[i] = g.shift != nullptr ? __ldg(g.shift + n_base + i) : 0.f;
   }
-  tc_fence_before_sync();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  __syncthreads();
+  cluster_sync_all();  // barriers of every CTA are initialised before any remote arrive
 
-  const int num_tiles = (g.m + 2 * kBlockM - 1) / (2 * kBlockM);
+  const int num_tiles = (g.m + kBlockM - 1) / kBlockM;
   const int num_kb = (g.k + kBlockK - 1) / kBlockK;
-  const int cluster_id = blockIdx.x / (2 * P);
-  const int num_clusters = gridDim.x / (2 * P);
+  const int cluster_id = blockIdx.x / C;
+  const int num_clusters = gridDim.x / C;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (every CTA): its 128 A rows, its 128 W rows of both accumulator halves =====
+  if (warp < 4) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      // ===== TMA producer: the cluster's 128 A rows, this CTA's 256 W rows =====
       uint32_t it = 0;
       for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        const int m0 = tile * (2 * kBlockM) + static_cast<int>(rank & 1u) * kBlockM;
-        const int n0 = n_base + static_cast<int>(rank & 1u) * kLoadN;
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const uint32_t s = it % kStages;
           mbar_wait(&empty_bar[s], ((it / kStages) & 1u) ^ 1u);
-          uint8_t* sb = smem_b + s * (2 * kSubB);
-          tma_load_2d_pair(smem_a + s * kStageBytesA, &tmap_a, &full_bar[s], kb * kBlockK, m0);
-          tma_load_2d_pair(sb, &tmap_w, &full_bar[s], kb * kBlockK, n0);
-          tma_load_2d_pair(sb + kSubB, &tmap_w, &full_bar[s], kb * kBlockK, n0 + kHalfN);
-          if (leader) mbar_arrive_expect_tx(&full_bar[s], 2 * kStageBytes);
-          else mbar_arrive_remote(&full_bar[s], pair_base);
+          mbar_arrive_expect_tx(&full_bar[s], kStageBytes);
+          tma_load_2d(smem_a + s * kStageBytesA, &tmap_a, &full_bar[s], kb * kBlockK, tile * kBlockM);
+          tma_load_2d(smem_b + s * kStageBytesB, &tmap_w, &full_bar[s], kb * kBlockK, n_base);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ===== MMA issuer (the leader CTA of every pair) =====
-      constexpr uint32_t idesc = umma_idesc_f16kind_f32(2 * kBlockM, kHalfN, kHalfIn);
-      uint32_t it = 0, tc = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tc) {
-        mbar_wait(tmem_empty_bar, (tc & 1u) ^ 1u);  // both CTAs have drained the previous tile out of TMEM
-        tc_fence_after_sync();
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const uint32_t s = it % kStages;
-          mbar_wait(&full_bar[s], (it / kStages) & 1u);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem_a + s * kStageBytesA);
-          const uint32_t b_addr = smem_u32(smem_b + s * (2 * kSubB));
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k)
-              umma_bf16_ss_pair(tmem_base + h * kHalfN, umma_desc_k_sw128(a_addr + k * kUmmaK * 2),
-                                umma_desc_k_sw128(b_addr + h * kSubB + k * kUmmaK * 2), idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_commit_pair_of(&empty_bar[s], pair_base);
-        }
-        umma_commit_pair_of(tmem_full_bar, pair_base);
-      }
-      if (tc > 0) mbar_wait(tmem_empty_bar, (tc - 1) & 1u);  // last remote arrivals land before the CTA may exit
-    }
-  } else if (warp == 3) {
-    // ===== residual prefetch into L2, one tile ahead of the epilogue =====
-    if (g.residual != nullptr) {
-      uint32_t tc = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tc) {
-        const int row0 = tile * (2 * kBlockM) + static_cast<int>(rank & 1u) * kBlockM;
-        for (int rr = lane; rr < kBlockM; rr += 32) {
-          const int row = row0 + rr;
-          if (row < g.m) {
-            const float* p = g.residual + static_cast<size_t>(row) * g.ldr + n_base;  // this pair's 2 KB of the row
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(kPairN * 4) : "memory");
-          }
-        }
-        mbar_wait(tmem_full_bar, tc & 1u);  // this tile's main loop is done: go and fetch the next tile's rows
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: thread = (row, 128-column group) =====
-    const int q = warp & 3;            // TMEM lane quadrant
-    const int cg = (warp - 4) >> 2;    // column group: columns [cg * 128, +128) of this pair's 512
-    const int r = q * 32 + lane;       // row inside this CTA's 128
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + cg * kColsPerWarp;  // accumulators are adjacent
+  } else {
+    // ===== math warpgroups =====
+    reg_alloc<232>();
+    const int wg = (warp >> 2) - 1;
+    const int t = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows inside the tile: r0, r0 + 8
     const float inv_n = 1.f / static_cast<float>(g.n);
-    const float* sb = s_bias + cg * kColsPerWarp;
-    const float* ssc = s_scale + cg * kColsPerWarp;
-    const float* ssh = s_shift + cg * kColsPerWarp;
-    const uint32_t stg = smem_u32(stage_out + (warp - 4) * kStageOutBytes);
-    const uint32_t st_row = stg + lane * 64;
-    const int sw_w = (lane >> 1) & 3;  // write side of the transpose tile: row = lane
-    const int rr = lane >> 2, jj = lane & 3;  // read side: 8 rows per instruction, 4 lanes (16 B each) per row
-    uint32_t tc = 0;
+    float acc[kCtaN / 2];
+    uint32_t it = 0, tc = 0;
     for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tc) {
-      mbar_wait(tmem_full_bar, tc & 1u);
-      tc_fence_after_sync();
-      // ---- pass 1: sum and sum of squares of y = acc + bias over this warp's 128 columns ----
+      int prev_s = -1;
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const uint32_t s = it % kStages;
+        mbar_wait(&full_bar[s], (it / kStages) & 1u);
+        const uint32_t a_addr = smem_u32(smem_a + s * kStageBytesA) + wg * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem_b + s * kStageBytesB);
+        wgmma_fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+          wgmma_ss<kCtaN, kHalfIn>(acc, wgmma_desc_sw128(a_addr + k * kWgmmaK * 2), wgmma_desc_sw128(b_addr + k * kWgmmaK * 2),
+                                   (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (prev_s >= 0) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
+        }
+        prev_s = static_cast<int>(s);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
+
+      // ---- 1. y = acc + bias, row sums over this CTA's 256 columns ----
       float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < kColsPerWarp; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + c, v);
-        tmem_ld_wait();
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 b4 = *reinterpret_cast<const float4*>(sb + c + j);
-          const float y0 = __uint_as_float(v[j]) + b4.x, y1 = __uint_as_float(v[j + 1]) + b4.y;
-          const float y2 = __uint_as_float(v[j + 2]) + b4.z, y3 = __uint_as_float(v[j + 3]) + b4.w;
-          s0 += y0 + y2;
-          s1 += y1 + y3;
-          q0 = fmaf(y0, y0, fmaf(y2, y2, q0));
-          q1 = fmaf(y1, y1, fmaf(y3, y3, q1));
-        }
+      for (int j = 0; j < kCtaN / 8; ++j) {
+        const float2 b = *reinterpret_cast<const float2*>(s_bias + 8 * j + 2 * t);
+        acc[4 * j + 0] += b.x, acc[4 * j + 1] += b.y, acc[4 * j + 2] += b.x, acc[4 * j + 3] += b.y;
+        s0 += acc[4 * j + 0] + acc[4 * j + 1];
+        s1 += acc[4 * j + 2] + acc[4 * j + 3];
+        q0 = fmaf(acc[4 * j + 0], acc[4 * j + 0], fmaf(acc[4 * j + 1], acc[4 * j + 1], q0));
+        q1 = fmaf(acc[4 * j + 2], acc[4 * j + 2], fmaf(acc[4 * j + 3], acc[4 * j + 3], q1));
       }
-      part[cg * 128 + r] = make_float2(s0 + s1, q0 + q1);
-      named_bar_sync(1 + q, 128);  // the four warps that share these 32 rows
-      float2 tot = part[r];
 #pragma unroll
-      for (int i = 1; i < 4; ++i) {
-        const float2 t = part[i * 128 + r];
-        tot.x += t.x, tot.y += t.y;
+      for (int o = 1; o <= 2; o <<= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+        q1 += __shfl_xor_sync(0xffffffffu, q1, o);
       }
-      if constexpr (P > 1) {
-        if (cg == 0) {
-          st_remote_f32(&rem[r].x, rank ^ 2u, tot.x);
-          st_remote_f32(&rem[r].y, rank ^ 2u, tot.y);
-          __syncwarp();
-          if (lane == 0) mbar_arrive_remote_release(stat_bar, rank ^ 2u);
-        }
-        mbar_wait_acquire_cluster(stat_bar, tc & 1u);
-        const float2 t = rem[r];
-        tot.x += t.x, tot.y += t.y;
+      // ---- 2. exchange with the CTAs that hold the other columns of these rows ----
+      float2* const slot = rem + (tc & 1u) * (kMaxCluster * kBlockM);
+      if (t == 0) {
+#pragma unroll
+        for (uint32_t c = 0; c < C; ++c)
+          if (c != rank) {
+            st_remote_f32x2(slot + rank * kBlockM + r0, c, make_float2(s0, q0));
+            st_remote_f32x2(slot + rank * kBlockM + r0 + 8, c, make_float2(s1, q1));
+          }
       }
-      const float mean = tot.x * inv_n;
-      const float rstd = rsqrtf(fmaxf(tot.y * inv_n - mean * mean, 0.f) + g.eps);
-      // ---- pass 2: normalise + modulate (thread = row), transpose through shared memory, then coalesced:
-      //      fp32 stream = residual + value, 16-bit copy ----
-      {
-        const int row_warp0 = tile * (2 * kBlockM) + static_cast<int>(rank & 1u) * kBlockM + q * 32;  // first row of this warp
-        const size_t col0 = static_cast<size_t>(n_base + cg * kColsPerWarp);
-#pragma unroll 1
-        for (int c = 0; c < kColsPerWarp; c += 16) {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(taddr + c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float4 b4 = *reinterpret_cast<const float4*>(sb + c + 4 * j);
-            const float4 sc4 = *reinterpret_cast<const float4*>(ssc + c + 4 * j);
-            const float4 sh4 = *reinterpret_cast<const float4*>(ssh + c + 4 * j);
-            const float f0 = fmaf((__uint_as_float(v[4 * j + 0]) + (b4.x - mean)) * rstd, sc4.x, sh4.x);
-            const float f1 = fmaf((__uint_as_float(v[4 * j + 1]) + (b4.y - mean)) * rstd, sc4.y, sh4.y);
-            const float f2 = fmaf((__uint_as_float(v[4 * j + 2]) + (b4.z - mean)) * rstd, sc4.z, sh4.z);
-            const float f3 = fmaf((__uint_as_float(v[4 * j + 3]) + (b4.w - mean)) * rstd, sc4.w, sh4.w);
-            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(st_row + ((j ^ sw_w) << 4)), "f"(f0), "f"(f1),
-                         "f"(f2), "f"(f3)
-                         : "memory");
-          }
-          __syncwarp();
-          float4 val[4], res[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {  // all four residual loads in flight before the first use
-            const int lr = i * 8 + rr;
-            const int grow = row_warp0 + lr;
-            res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (grow < g.m && g.residual != nullptr)
-              res[i] = *reinterpret_cast<const float4*>(g.residual + static_cast<size_t>(grow) * g.ldr + col0 + c + 4 * jj);
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int lr = i * 8 + rr;
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                         : "=f"(val[i].x), "=f"(val[i].y), "=f"(val[i].z), "=f"(val[i].w)
-                         : "r"(stg + lr * 64 + ((jj ^ ((lr >> 1) & 3)) << 4)));
-          }
-          __syncwarp();  // every lane has read the tile: the next chunk may overwrite it while the stores drain
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int grow = row_warp0 + i * 8 + rr;
-            if (grow < g.m) {
-              const size_t col = col0 + c + 4 * jj;
-              float4 o = val[i];
-              o.x += res[i].x, o.y += res[i].y, o.z += res[i].z, o.w += res[i].w;
-              if (g.out_f32 != nullptr) *reinterpret_cast<float4*>(g.out_f32 + static_cast<size_t>(grow) * g.ld_f32 + col) = o;
-              if (g.out_16 != nullptr) {
-                uint2 p;
-                if (g.out_half) p.x = pack_f16x2(o.x, o.y), p.y = pack_f16x2(o.z, o.w);
-                else p.x = pack_bf16x2(o.x, o.y), p.y = pack_bf16x2(o.z, o.w);
-                *reinterpret_cast<uint2*>(g.out_16 + static_cast<size_t>(grow) * g.ld_16 + col) = p;
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before_sync();
       __syncwarp();
-      if (lane == 0) mbar_arrive_remote(tmem_empty_bar, pair_base);  // the pair leader's barrier collects both CTAs
+      if (lane == 0) {
+#pragma unroll
+        for (uint32_t c = 0; c < C; ++c)
+          if (c != rank) mbar_arrive_remote_release(&stat_bar[tc & 1u], c);
+      }
+      mbar_wait_acquire_cluster(&stat_bar[tc & 1u], (tc >> 1) & 1u);
+#pragma unroll
+      for (uint32_t c = 0; c < C; ++c)
+        if (c != rank) {
+          const float2 a0 = slot[c * kBlockM + r0], a1 = slot[c * kBlockM + r0 + 8];
+          s0 += a0.x, q0 += a0.y, s1 += a1.x, q1 += a1.y;
+        }
+      const float mean0 = s0 * inv_n, mean1 = s1 * inv_n;
+      const float rstd0 = rsqrtf(fmaxf(q0 * inv_n - mean0 * mean0, 0.f) + g.eps);
+      const float rstd1 = rsqrtf(fmaxf(q1 * inv_n - mean1 * mean1, 0.f) + g.eps);
+      // ---- 3. normalise + modulate + residual -> fp32 stream, 16-bit copy ----
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = tile * kBlockM + r0 + 8 * h;
+        if (row >= g.m) continue;
+        const float mean = h ? mean1 : mean0, rstd = h ? rstd1 : rstd0;
+#pragma unroll
+        for (int j = 0; j < kCtaN / 8; ++j) {
+          const int cl = 8 * j + 2 * t;
+          const float2 sc = *reinterpret_cast<const float2*>(s_scale + cl);
+          const float2 sh = *reinterpret_cast<const float2*>(s_shift + cl);
+          float2 o;
+          o.x = fmaf((acc[4 * j + 2 * h] - mean) * rstd, sc.x, sh.x);
+          o.y = fmaf((acc[4 * j + 2 * h + 1] - mean) * rstd, sc.y, sh.y);
+          const size_t col = static_cast<size_t>(n_base + cl);
+          if (g.residual != nullptr) {
+            const float2 r = *reinterpret_cast<const float2*>(g.residual + static_cast<size_t>(row) * g.ldr + col);
+            o.x += r.x, o.y += r.y;
+          }
+          if (g.out_f32 != nullptr) *reinterpret_cast<float2*>(g.out_f32 + static_cast<size_t>(row) * g.ld_f32 + col) = o;
+          if (g.out_16 != nullptr)
+            *reinterpret_cast<uint32_t*>(g.out_16 + static_cast<size_t>(row) * g.ld_16 + col) =
+                g.out_half ? pack_f16x2(o.x, o.y) : pack_bf16x2(o.x, o.y);
+        }
+      }
     }
   }
-
+  // no CTA may exit while a neighbour can still store into its shared memory
   __syncwarp();
-  tc_fence_before_sync();
   cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc_pair<512>(tmem_base);
-  }
 }
 
-template <bool kHalfIn, int P>
+template <bool kHalfIn, int C>
 static int launch(const AbGemmLn* p, const Args& a, cudaStream_t stream) {
   CUtensorMap ta, tw;
   int rc = make_tmap_16bit_2d(&ta, p->a, p->m, p->k, p->lda, kBlockM, kBlockK, kHalfIn);
   if (rc != AB_OK) return rc;
-  rc = make_tmap_16bit_2d(&tw, p->w, p->n, p->k, p->ldw, kLoadN, kBlockK, kHalfIn);
+  rc = make_tmap_16bit_2d(&tw, p->w, p->n, p->k, p->ldw, kCtaN, kBlockK, kHalfIn);
   if (rc != AB_OK) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_ln_kernel<kHalfIn, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(gemm_ln_kernel<kHalfIn, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
     if (e != cudaSuccess) {
       set_error("ab_gemm_ln_residual: cudaFuncSetAttribute(smem=%d) failed: %s", kSmemBytes, cudaGetErrorString(e));
       return AB_ERR_CUDA;
     }
     attr_set = true;
   }
-  const long long tiles = ceil_div_ll(p->m, 2 * kBlockM);
-  const long long max_clusters = sm_count() / (2 * P);
+  const long long tiles = ceil_div_ll(p->m, kBlockM);
+  const long long max_clusters = sm_count() / C;
   const int clusters = static_cast<int>(tiles < max_clusters ? tiles : max_clusters);
-  gemm_ln_kernel<kHalfIn, P><<<2 * P * clusters, kThreads, kSmemBytes, stream>>>(ta, tw, a);
+  gemm_ln_kernel<kHalfIn, C><<<C * clusters, kThreads, kSmemBytes, stream>>>(ta, tw, a);
   AB_COUNT_LAUNCH(1);
   AB_CHECK_LAUNCH("ab_gemm_ln_residual");
   return AB_OK;
@@ -432,6 +327,6 @@ extern "C" int ab_gemm_ln_residual(const AbGemmLn* p, void* stream) {
   a.eps = p->eps;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const bool half_in = p->in_dtype == AB_DT_F16;
-  if (p->n == 512) return half_in ? gln::launch<true, 1>(p, a, s) : gln::launch<false, 1>(p, a, s);
-  return half_in ? gln::launch<true, 2>(p, a, s) : gln::launch<false, 2>(p, a, s);
+  if (p->n == 512) return half_in ? gln::launch<true, 2>(p, a, s) : gln::launch<false, 2>(p, a, s);
+  return half_in ? gln::launch<true, 4>(p, a, s) : gln::launch<false, 4>(p, a, s);
 }

@@ -1,4 +1,5 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors, clusters.
+// The wgmma.mma_async wrappers themselves are in wgmma.cuh.
 // Everything here is hand-written PTX; no CUTLASS/CuTe dependency.
 #pragma once
 
@@ -124,110 +125,37 @@ constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
 constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, TMEM loads
+// wgmma operand descriptors, register budget
 // ---------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: pow2 in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes with the
-// 128-byte swizzle (what a TMA box of {64 bf16, rows} with CU_TENSOR_MAP_SWIZZLE_128B produces).
+// Shared-memory matrix descriptor for an operand tile stored as rows of 128 bytes with the 128-byte swizzle (what a
+// TMA box of {64 16-bit elements, rows} with CU_TENSOR_MAP_SWIZZLE_128B produces), 1024-byte aligned.
 //   start address  : bits [0,14)   (bytes >> 4)
-//   leading offset : bits [16,30)  (unused for swizzled K-major; canonical value 1)
+//   leading offset : bits [16,30)  (unused for one 128-byte swizzle atom per row; canonical value 1)
 //   stride offset  : bits [32,46)  (bytes >> 4 between 8-row groups = 1024 B)
-//   version        : bits [46,48)  = 1 on sm_100
-//   layout type    : bits [61,64)  = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr_bytes) {
+//   layout type    : bits [62,64)  = 1 (SWIZZLE_128B)
+// K-major operands advance along K by adding the byte offset inside the 128-byte row to the start address; an
+// MN-major operand (wgmma's transposed-B form) advances along K by whole 8-row groups.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr_bytes & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16 with bf16 (or fp16) A/B, K-major both, fp32 accumulation.
-__host__ __device__ constexpr uint32_t umma_idesc_f16kind_f32(uint32_t m, uint32_t n, bool fp16_operands) {
-  return (1u << 4)                              // D format: F32
-         | ((fp16_operands ? 0u : 1u) << 7)     // A format: F16 = 0, BF16 = 1
-         | ((fp16_operands ? 0u : 1u) << 10)    // B format
-         | ((n >> 3) << 17)                     // N / 8
-         | ((m >> 4) << 24);                    // M / 16
+// Register hand-over between warpgroups: the producer warpgroup gives registers up, the math warpgroups take them.
+template <int kRegs>
+__device__ __forceinline__ void reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+template <int kRegs>
+__device__ __forceinline__ void reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
-
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread t gets lane t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-
-// TMEM -> registers, 16 / 32 consecutive fp32 columns of this warp's 32 lanes.
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// Same as umma_idesc_f16kind_f32 with the B operand MN-major (rows of B^T contiguous in N): used for P.V
-// where V is stored [key][d] (d contiguous).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_bmn(uint32_t m, uint32_t n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
-// Thread-block clusters / CTA pairs (cta_group::2)
+// Thread-block clusters
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -237,58 +165,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster.
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 remaddr;\n\t"
-      "mapa.shared::cluster.u32 remaddr, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [remaddr];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// TMA load issued by either CTA of a pair; the transaction bytes are credited to the LEADER CTA's
-// mbarrier (peer bit of the barrier address cleared).
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar,
-                                                 int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem of both CTAs] * B[smem halves of both CTAs]^T, M = 256; leader CTA only.
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once the pair's MMAs issued so far retire) on the mbarrier at this offset in BOTH CTAs.
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -349,8 +225,8 @@ __device__ __forceinline__ uint16_t to16(float x, int half) {
 //   gelu(x) = max(x, 0) - |x| * h(z),  z = |x| / sqrt(2),  h(z) = 0.5 erfc(z) = exp(-z^2) * R(z)
 // with R a degree-6 minimax fit of 0.5 * erfcx on [0, 4.5] (z clamped there; erfc(4.5) = 2e-10).
 // Max abs error 1.4e-5 over all x (fit: tools/fit_gelu.py) — far below the 16-bit rounding of the stored
-// activation — for 13 ALU ops + 1 MUFU.  erff() costs ~30 instructions and made fc1's epilogue the
-// bottleneck: at K = 512 the tensor pipe produces 8 outputs / clk / SM, i.e. 16 issue slots per element.
+// activation — for 13 ALU ops + 1 MUFU, against ~30 instructions for erff(): the fc1 epilogue runs on the same
+// warps that issue the next tile's wgmma, so every instruction saved here is tensor-pipe time.
 __device__ __forceinline__ float gelu_erf(float x) {
   const float z = fminf(fabsf(x) * 0.70710678118654752440f, 4.5f);
   float e;
@@ -362,53 +238,6 @@ __device__ __forceinline__ float gelu_erf(float x) {
   r = fmaf(r, z, -0.5599349141120911f);
   r = fmaf(r, z, 0.49980518221855164f);
   return fmaf(-fabsf(x), e * r, fmaxf(x, 0.f));
-}
-
-// Two GELUs at once on the packed fp32 pipe (fma / mul .f32x2, sm_100+): same polynomial and rounding as
-// gelu_erf, 9 instead of 14.5 issue slots per element.  The K = 512 fc1 epilogue is bound by the issue slots
-// of its 8 epilogue warps (profiles/r01_ncu_full_summaries.md, r01h), so this is what the tensor pipe waits for.
-__device__ __forceinline__ uint64_t f32x2_pack(float a, float b) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void f32x2_unpack(uint64_t v, float& a, float& b) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f32x2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ uint64_t f32x2_mul(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t f32x2_add(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t f32x2_splat(float c) { return f32x2_pack(c, c); }
-
-__device__ __forceinline__ void gelu_erf_x2(float& x0, float& x1) {
-  const float na0 = -fabsf(x0), na1 = -fabsf(x1);
-  const float z0 = fminf(na0 * -0.70710678118654752440f, 4.5f);
-  const float z1 = fminf(na1 * -0.70710678118654752440f, 4.5f);
-  const uint64_t z = f32x2_pack(z0, z1);
-  float a0, a1, e0, e1;
-  f32x2_unpack(f32x2_mul(f32x2_mul(z, f32x2_splat(-1.4426950408889634f)), z), a0, a1);
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(a0));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-  uint64_t r = f32x2_fma(f32x2_splat(0.003532303497195244f), z, f32x2_splat(-0.032581403851509094f));
-  r = f32x2_fma(r, z, f32x2_splat(0.12916485965251923f));
-  r = f32x2_fma(r, z, f32x2_splat(-0.29942014813423157f));
-  r = f32x2_fma(r, z, f32x2_splat(0.47322216629981995f));
-  r = f32x2_fma(r, z, f32x2_splat(-0.5599349141120911f));
-  r = f32x2_fma(r, z, f32x2_splat(0.49980518221855164f));
-  const uint64_t er = f32x2_mul(f32x2_pack(e0, e1), r);
-  f32x2_unpack(f32x2_fma(f32x2_pack(na0, na1), er, f32x2_pack(fmaxf(x0, 0.f), fmaxf(x1, 0.f))), x0, x1);
 }
 
 }  // namespace ab

@@ -19,6 +19,7 @@
 
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 #include "window_index.cuh"
 
 namespace ab {
@@ -348,39 +349,37 @@ __global__ void __launch_bounds__(kAttnThreads, 2) window_attention_kernel(const
 
 
 // ================================================================================================
-// tcgen05 / TMEM attention for FULL windows (2 x 6 x 12 = 144 tokens, head_dim 64): the production case.
+// wgmma attention for FULL windows (2 x 6 x 12 = 144 tokens, head_dim 64): the production case.
 //
 // Persistent CTA per SM, warp-specialised, one (window, head) item per pipeline slot:
-//   warps 0-1 : loaders.  Warp w handles items n = w (mod 2): index map + group ids by closed form
-//               (window_index.cuh), then a TMA ROW-BOX GATHER of the window's q / k / v rows into a FOUR-stage
-//               128B-swizzled ring (bias rows for zero-padded tokens are filled by the warp itself).
-//   warp 2    : MMA issuer (one lane).  S = Q K^T as two M=128 x N=144 x K=64 tcgen05.mma tiles (rows 0-127 and
-//               32-159 of the Q tile; rows >= 144 are don't-care), accumulators in TMEM; O = P V as two
-//               M=128 x N=64 x K=144 tiles with **P AS THE TMEM A OPERAND** (`tcgen05.mma [d], [a_tmem], b_desc`) and
-//               V as an MN-major B operand straight from the gathered [key][d] rows.  S0(n+1) is issued as soon as
-//               the tile-0 warps hold S0(n) in registers; S1(n+1) after P V(n), because P of tile 1 lives in the
-//               first 72 columns of S1 and the tensor pipe executes in issue order.
-//   warps 3-7 : softmax + epilogue, ONE THREAD PER QUERY ROW (TMEM lane = row): tcgen05.ld the 144 logits, add
-//               the 0 / -100 shifted-window mask from one byte of group id per key, max / exp2 / sum without any
-//               shuffle, write P (bf16 pairs) back to TMEM with tcgen05.st — no shared-memory round trip, no
-//               generic->async proxy fence — and, one item later, read O, scale by 1 / sum and store the 128-byte
-//               output row at the source token (reverse + crop + un-roll).
-// History (profiles/r01p_ncu_final_captures.md, r02 probe): the round-1 kernel wrote P to swizzled shared memory
-// (26 % of the softmax warps' samples in STS + fence) with a three-stage ring; P in TMEM + the 4th stage in the freed
-// 54 KB measured 7-12 % faster on the three stage grids, bit-identical output.
+//   warpgroup 0    : loaders (warps 0-1; registers handed to the math warpgroups).  Warp w handles items n = w (mod 2):
+//                    index map + group ids by closed form (window_index.cuh), then a TMA ROW-BOX GATHER of the window's
+//                    q / k / v rows into a FOUR-stage 128B-swizzled ring (bias rows for zero-padded tokens are filled
+//                    by the warp itself).
+//   warpgroups 1-3 : math.  Warpgroup g owns query rows [64 g, 64 g + 64) (wgmma's M is 64: rows >= 144 of the third
+//                    warpgroup are don't-care and never stored; the kernel is HBM-bound, the idle tensor rows are free).
+//                    S = Q K^T as four m64n144k16 wgmmas, both operands straight from the swizzled stage, the 64 x 144
+//                    logits in registers; 0 / -100 shifted-window mask from one byte of group id per key, max / exp2 /
+//                    sum with two quad shuffles per row; P stays IN REGISTERS — the fp32 accumulator fragment of S,
+//                    packed to bf16 pairs, is exactly the A fragment of the next wgmma — and O = P V runs as nine
+//                    m64n64k16 wgmmas with A from registers and V as the transposed (MN-major) B operand straight from
+//                    the gathered [key][d] rows.  O is scaled by 1 / sum, staged in the warp's own (now dead) Q rows and
+//                    stored as 128-byte rows at the source tokens (reverse + crop + un-roll).
+// The three warpgroups run the same item on different rows without synchronising with each other, so one warpgroup's
+// softmax overlaps the others' tensor work; the ring lets the loaders run up to three items ahead.
 // ================================================================================================
 namespace tc {
 
 constexpr int kTok = 144;
 constexpr int kTileBytes = kTok * kRowBytes;       // 18 KB per q / k / v tile
 constexpr int kStageBytes = 3 * kTileBytes;        // 54 KB
-constexpr int kStages = 4;                         // q/k/v ring: a stage is only released by P V, loads must run ahead
+constexpr int kStages = 4;                         // q/k/v ring: a stage is only released after P V, loads must run ahead
 constexpr int kOffMeta = kStages * kStageBytes;    // 216 KB
 constexpr int kMetaBytes = 6144;
 constexpr int kSmemBytes = kOffMeta + kMetaBytes + 1024;
 static_assert(kSmemBytes <= 227 * 1024, "shared memory");
-constexpr int kThreads = 8 * 32;  // two warps per scheduler: every thread may use up to 255 registers
-constexpr int kTile1Row0 = 32;    // tile 1 covers Q rows 32..159, so rows 128..143 sit in TMEM lanes 96..111 (warp 3)
+constexpr int kMathWarps = 12;    // three warpgroups x 64 query rows
+constexpr int kThreads = 128 + kMathWarps * 32;
 
 // win_source_token() for the fixed (2, 6, 12) window with the window already decoded to (k0, k1, k2):
 // compile-time divisors only (the generic routine's runtime divisions made the single loader warp the
@@ -480,9 +479,6 @@ __device__ __forceinline__ void tc_translate(const AttnArgs& a, int src, int* lo
   *load_row = kHaloFlag | (((g.res[0] + c) * a.halo + down) * g.res[2] + w);  // host guarantees down < halo
 }
 
-// TMEM columns (all multiples of 16): S0 [0,144)  P0 [144,216)  O0 [224,288)  S1 [288,432) with P1 = [288,360)  O1 [432,496)
-constexpr uint32_t kColS0 = 0, kColP0 = 144, kColO0 = 224, kColS1 = 288, kColP1 = kColS1, kColO1 = 432;
-
 struct Meta {
   int lsrc[kStages][kTok];
   int src[kStages][kTok];
@@ -490,42 +486,9 @@ struct Meta {
   int masked[kStages];
   int head[kStages];
   int batch[kStages];
-  uint64_t full[kStages], empty[kStages], s0_full, s1_full, s0_free, p_full, o_full, o_free;
-  uint32_t tmem_slot;
+  uint64_t full[kStages], empty[kStages];
 };
 static_assert(sizeof(Meta) <= kMetaBytes, "meta area");
-
-// D[tmem] (+)= A[tmem] * B[smem]^T : A = 128 lanes x 8 columns of packed 16-bit pairs (K = 16) per instruction.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// registers -> TMEM: this warp's 32 lanes x 32 / 8 consecutive 32-bit columns (thread t writes lane t).
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // Wait until both neighbours' halo pushes of the current round have landed (protocol: csrc/halo.cu).  ctrl[0] / ctrl[1]
 // are written by the ranks above / below with st.release.sys, ctrl[2] is this rank's own round (its push precedes this
@@ -552,8 +515,7 @@ __device__ __forceinline__ void halo_wait_flags(const uint32_t* ctrl, int lane) 
 __global__ void __launch_bounds__(kThreads, 1)
 window_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_halo,
                            const AttnArgs a) {
-  // warps: 0-1 loaders, 2 MMA issuer (+ barrier init, TMEM alloc), 3 softmax of rows 128..143 (TMEM lane
-  // quadrant 3 of tile 1), 4-7 softmax of rows 0..127 (quadrants 0..3 of tile 0).
+  // warps: 0-1 loaders (2-3 idle), 4-15 math: warp w holds query rows [16 (w - 4), 16 (w - 4) + 16).
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   Meta* meta = reinterpret_cast<Meta*>(smem + kOffMeta);
@@ -570,24 +532,13 @@ window_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const _
   if (warp == 2 && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&meta->full[i], 1);
-      mbar_init(&meta->empty[i], 1);
+      mbar_init(&meta->empty[i], kMathWarps);
     }
-    mbar_init(&meta->s0_full, 1);
-    mbar_init(&meta->s1_full, 1);
-    mbar_init(&meta->s0_free, 4);  // only the four tile-0 warps release S0 (S1 is re-issued after P V, in pipe order)
-    mbar_init(&meta->p_full, 5);
-    mbar_init(&meta->o_full, 1);
-    mbar_init(&meta->o_free, 5);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    __syncwarp();
-    tmem_alloc<512>(&meta->tmem_slot);
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = meta->tmem_slot;
+  if (warp < 4) reg_dealloc<40>();
+  else reg_alloc<152>();
 
   if (warp < 2) {
     // ===== loaders: warp w takes items n = w (mod 2); item n lives in ring stage n % kStages =====
@@ -677,7 +628,7 @@ window_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const _
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) bytes += __shfl_xor_sync(0xffffffffu, bytes, o);
-        fence_proxy_async_smem();  // bias fills (generic proxy) -> tensor core
+        fence_proxy_async_smem();  // bias fills (generic proxy) -> wgmma (async proxy)
         __syncwarp();
         if (lane == 0) mbar_arrive_expect_tx(&meta->full[st], bytes);
         continue;
@@ -700,215 +651,117 @@ window_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const _
         cp_async_16(sv + off, p + 2 * a.dim);
       }
       cp_async_wait_all();
-      fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
+      fence_proxy_async_smem();  // generic-proxy writes -> visible to wgmma (async proxy)
       __syncwarp();
       if (lane == 0) mbar_arrive(&meta->full[st]);
     }
-  } else if (warp == 2) {
-    if (lane == 0 && cnt > 0) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc_s = umma_idesc_f16kind_f32(128, kTok, false);
-      constexpr uint32_t idesc_o = umma_idesc_bf16_bmn(128, kHeadDim);  // A (now in TMEM) K-major, B = V MN-major
-      // S tile 0 and S tile 1 are issued (and signalled) separately.  S0(n+1) goes out as soon as the tile-0
-      // warps hold S0(n) in registers (tensor work under the softmax, as before); S1(n+1) is issued AFTER P V(n),
-      // because P of tile 1 lives in the first 72 columns of S1 and tcgen05.mma executes in issue order.
-      auto issue_s0 = [&](int n) {
-        const uint32_t qa = smem_u32(smem + (n % kStages) * kStageBytes);
-        const uint32_t ka = qa + kTileBytes;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16_ss(tmem_base + kColS0, umma_desc_k_sw128(qa + k * 32), umma_desc_k_sw128(ka + k * 32), idesc_s, k != 0);
-        umma_commit(&meta->s0_full);
-      };
-      auto issue_s1 = [&](int n) {
-        const uint32_t qa = smem_u32(smem + (n % kStages) * kStageBytes);
-        const uint32_t ka = qa + kTileBytes;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16_ss(tmem_base + kColS1, umma_desc_k_sw128(qa + kTile1Row0 * kRowBytes + k * 32),
-                       umma_desc_k_sw128(ka + k * 32), idesc_s, k != 0);
-        umma_commit(&meta->s1_full);
-      };
-      mbar_wait(&meta->full[0], 0);
-      tc_fence_after_sync();
-      issue_s0(0);
-      issue_s1(0);
-      for (int n = 0; n < cnt; ++n) {
-        if (n + 1 < cnt) {
-          mbar_wait(&meta->full[(n + 1) % kStages], ((n + 1) / kStages) & 1);
-          mbar_wait(&meta->s0_free, n & 1);  // the tile-0 softmax warps have pulled S0(n) out of TMEM
-          tc_fence_after_sync();
-          issue_s0(n + 1);
-        }
-        mbar_wait(&meta->p_full, n & 1);     // P(n) is in TMEM (tcgen05.st + wait::st + fence on the writer side)
-        if (n > 0) mbar_wait(&meta->o_free, (n - 1) & 1);
-        tc_fence_after_sync();
-        const uint32_t va = smem_u32(smem + (n % kStages) * kStageBytes) + 2 * kTileBytes;
-#pragma unroll
-        for (int j = 0; j < kTok / 16; ++j) {  // 9 k-steps of 16 keys = 8 TMEM columns of packed bf16 pairs each
-          const uint64_t dv = umma_desc_k_sw128(va + j * 16 * kRowBytes);
-          umma_bf16_ts(tmem_base + kColO0, tmem_base + kColP0 + j * 8, dv, idesc_o, j != 0);
-          umma_bf16_ts(tmem_base + kColO1, tmem_base + kColP1 + j * 8, dv, idesc_o, j != 0);
-        }
-        umma_commit(&meta->o_full);
-        umma_commit(&meta->empty[n % kStages]);  // q / k / v of this stage are consumed
-        if (n + 1 < cnt) issue_s1(n + 1);        // overwrites P1(n) only after P V(n) above has read it
-      }
-    }
-  } else {
-    // ===== softmax + epilogue (warps 3..7): thread = query row =====
-    const int tile = (warp == 3) ? 1 : 0;
-    const int lrow = (warp & 3) * 32 + lane;           // row inside the tile (TMEM lane)
-    const int row = tile * kTile1Row0 + lrow;          // window token
-    const bool valid = row < kTok;
-    const uint32_t lane_addr = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t s_addr = tmem_base + lane_addr + (tile ? kColS1 : kColS0);
-    const uint32_t o_addr = tmem_base + lane_addr + (tile ? kColO1 : kColO0);
-    // P goes to TMEM (this thread's lane, 72 columns of packed bf16 pairs): tile 0 has its own columns, tile 1
-    // reuses the first 72 columns of its S tile.
-    const uint32_t p_addr = tmem_base + lane_addr + (tile ? kColP1 : kColP0);
-    uint64_t* const my_s_full = tile ? &meta->s1_full : &meta->s0_full;
+  } else if (warp >= 4) {
+    // ===== math warpgroups =====
+    const int wg = (warp >> 2) - 1;
+    const int row_w = (warp - 4) * 16;      // first query row of this warp
+    const bool active = row_w < kTok;       // warp-uniform; 144 = 9 x 16, so an active warp holds 16 real rows
+    const int t = lane & 3;
+    const int qrow0 = row_w + (lane >> 2), qrow1 = qrow0 + 8;
     constexpr float kC = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) in the exp2 domain
-
-    int prev_src = -1;
-    float prev_inv = 0.f;
-    int prev_b = 0, prev_head = 0;
-    auto epilogue = [&](int n_prev) {
-      mbar_wait(&meta->o_full, n_prev & 1);
-      tc_fence_after_sync();
-      uint32_t o0[32], o1[32];
-      tmem_ld_32x32b_x32(o_addr, o0);
-      tmem_ld_32x32b_x32(o_addr + 32, o1);
-      tmem_ld_wait();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&meta->o_free);
-      if (valid && prev_src >= 0) {
-        uint4* dst = reinterpret_cast<uint4*>(a.out + (static_cast<long long>(prev_b) * a.tokens_per_batch + prev_src) * a.dim +
-                                              prev_head * kHeadDim);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4 u;
-          u.x = pack_bf16x2(__uint_as_float(o0[8 * c + 0]) * prev_inv, __uint_as_float(o0[8 * c + 1]) * prev_inv);
-          u.y = pack_bf16x2(__uint_as_float(o0[8 * c + 2]) * prev_inv, __uint_as_float(o0[8 * c + 3]) * prev_inv);
-          u.z = pack_bf16x2(__uint_as_float(o0[8 * c + 4]) * prev_inv, __uint_as_float(o0[8 * c + 5]) * prev_inv);
-          u.w = pack_bf16x2(__uint_as_float(o0[8 * c + 6]) * prev_inv, __uint_as_float(o0[8 * c + 7]) * prev_inv);
-          dst[c] = u;
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4 u;
-          u.x = pack_bf16x2(__uint_as_float(o1[8 * c + 0]) * prev_inv, __uint_as_float(o1[8 * c + 1]) * prev_inv);
-          u.y = pack_bf16x2(__uint_as_float(o1[8 * c + 2]) * prev_inv, __uint_as_float(o1[8 * c + 3]) * prev_inv);
-          u.z = pack_bf16x2(__uint_as_float(o1[8 * c + 4]) * prev_inv, __uint_as_float(o1[8 * c + 5]) * prev_inv);
-          u.w = pack_bf16x2(__uint_as_float(o1[8 * c + 6]) * prev_inv, __uint_as_float(o1[8 * c + 7]) * prev_inv);
-          dst[4 + c] = u;
-        }
-      }
-    };
-
     for (int n = 0; n < cnt; ++n) {
       const int st = n % kStages;
-      mbar_wait(&meta->full[st], (n / kStages) & 1);  // index map / group ids of this item are in smem
-      const int my_src = valid ? meta->src[st][row] : -1;
-      const int my_grp = valid ? meta->grp[st][row] : 0;
-      const int masked = meta->masked[st];
-      const int cur_b = meta->batch[st], cur_head = meta->head[st];
-      mbar_wait(my_s_full, n & 1);
-      tc_fence_after_sync();
-      float sv[kTok];
-      {
-        uint32_t t0[32], t1[32], t2[32], t3[32], t4[16];
-        tmem_ld_32x32b_x32(s_addr, t0);
-        tmem_ld_32x32b_x32(s_addr + 32, t1);
-        tmem_ld_32x32b_x32(s_addr + 64, t2);
-        tmem_ld_32x32b_x32(s_addr + 96, t3);
-        tmem_ld_32x32b_x16(s_addr + 128, t4);
-        tmem_ld_wait();
+      uint8_t* const stage = smem + st * kStageBytes;
+      mbar_wait(&meta->full[st], (n / kStages) & 1);
+      const uint32_t qa = smem_u32(stage) + wg * (64 * kRowBytes);
+      const uint32_t ka = smem_u32(stage) + kTileBytes, va = ka + kTileBytes;
+      float sv[kTok / 2];  // [4 j + 2 h + e]: row qrow_h, key 8 j + 2 t + e
+      wgmma_fence_regs(sv);
+      wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          sv[j] = __uint_as_float(t0[j]);
-          sv[32 + j] = __uint_as_float(t1[j]);
-          sv[64 + j] = __uint_as_float(t2[j]);
-          sv[96 + j] = __uint_as_float(t3[j]);
-        }
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<kTok, false>(sv, wgmma_desc_sw128(qa + k * 32), wgmma_desc_sw128(ka + k * 32), k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(sv);
+      uint32_t pa[kTok / 16][4];
+      float inv0 = 0.f, inv1 = 0.f;
+      if (active) {
+        if (meta->masked[st]) {
+          // 0 / -100 on the scaled logits == 0 / -800 on the raw q.k products (scale 1/8)
+          const uint8_t* grp = meta->grp[st];
+          const int gq0 = grp[qrow0], gq1 = grp[qrow1];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) sv[128 + j] = __uint_as_float(t4[j]);
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0 && tile == 0) mbar_arrive(&meta->s0_free);  // S(n) is in registers: S(n+1) may overwrite it
-      if (masked) {
-        // 0 / -100 on the scaled logits == 0 / -800 on the raw q.k products (scale 1/8)
-        const uint4* g16 = reinterpret_cast<const uint4*>(meta->grp[st]);
-        const uint32_t mine = static_cast<uint32_t>(my_grp) * 0x01010101u;
-#pragma unroll
-        for (int w16 = 0; w16 < kTok / 16; ++w16) {
-          const uint4 gv = g16[w16];  // broadcast load: sixteen keys' group ids
-          const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w};
-#pragma unroll
-          for (int w4 = 0; w4 < 4; ++w4) {
-            const uint32_t ne = __vcmpne4(gw[w4], mine);  // 0xff per key of another group
-            const int j = 16 * w16 + 4 * w4;
-            if (ne & 0x000000ffu) sv[j] -= 800.f;
-            if (ne & 0x0000ff00u) sv[j + 1] -= 800.f;
-            if (ne & 0x00ff0000u) sv[j + 2] -= 800.f;
-            if (ne & 0xff000000u) sv[j + 3] -= 800.f;
+          for (int j = 0; j < kTok / 8; ++j) {
+            const uint16_t gk2 = *reinterpret_cast<const uint16_t*>(grp + 8 * j + 2 * t);  // two adjacent keys
+            const int gk_a = gk2 & 0xff, gk_b = gk2 >> 8;
+            if (gk_a != gq0) sv[4 * j + 0] -= 800.f;
+            if (gk_b != gq0) sv[4 * j + 1] -= 800.f;
+            if (gk_a != gq1) sv[4 * j + 2] -= 800.f;
+            if (gk_b != gq1) sv[4 * j + 3] -= 800.f;
           }
         }
-      }
-      float mxa[4] = {sv[0], sv[1], sv[2], sv[3]};  // four independent chains: one warp per scheduler has no TLP
+        float mx0 = fmaxf(sv[0], sv[1]), mx1 = fmaxf(sv[2], sv[3]);
 #pragma unroll
-      for (int j = 4; j < kTok; ++j) mxa[j & 3] = fmaxf(mxa[j & 3], sv[j]);
-      const float mx = fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3]));
-      const float nm = -mx * kC;
-      float suma[4] = {0.f, 0.f, 0.f, 0.f};
-      uint32_t pk[kTok / 2];
-#pragma unroll
-      for (int j = 0; j < kTok / 2; ++j) {
-        const float e0 = ex2_approx(fmaf(sv[2 * j], kC, nm));
-        const float e1 = ex2_approx(fmaf(sv[2 * j + 1], kC, nm));
-        suma[j & 3] += e0 + e1;
-        pk[j] = pack_bf16x2(e0, e1);
-      }
-      const float sum = (suma[0] + suma[1]) + (suma[2] + suma[3]);
-      // P(n) may only replace P(n-1) once P V(n-1) has retired; that is what o_full(n-1) says.  Doing the
-      // previous item's epilogue here keeps the tensor pipe busy with P V(n-1) / S(n+1) under this softmax.
-      if (n > 0) epilogue(n - 1);
-      // P(n) -> TMEM.  tcgen05.st is warp-collective: every lane stores (rows >= 144 hold don't-care values whose
-      // accumulator rows are never read).  P0(n) may replace P0(n-1) because epilogue(n-1) above has waited for
-      // o_full(n-1), i.e. P V(n-1) has retired; P1(n) goes over S1(n), which this thread has already pulled out.
-      {
-        uint32_t c0[32], c1[32], c2[8];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          c0[j] = pk[j];
-          c1[j] = pk[32 + j];
+        for (int j = 1; j < kTok / 8; ++j) {
+          mx0 = fmaxf(mx0, fmaxf(sv[4 * j + 0], sv[4 * j + 1]));
+          mx1 = fmaxf(mx1, fmaxf(sv[4 * j + 2], sv[4 * j + 3]));
         }
+        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+        const float nm0 = -mx0 * kC, nm1 = -mx1 * kC;
+        float sum0 = 0.f, sum1 = 0.f;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) c2[j] = pk[64 + j];
-        tmem_st_32x32b_x32(p_addr, c0);
-        tmem_st_32x32b_x32(p_addr + 32, c1);
-        tmem_st_32x32b_x8(p_addr + 64, c2);
-        tmem_st_wait();
+        for (int j = 0; j < kTok / 8; ++j) {
+          const float p0 = ex2_approx(fmaf(sv[4 * j + 0], kC, nm0)), p1 = ex2_approx(fmaf(sv[4 * j + 1], kC, nm0));
+          const float p2 = ex2_approx(fmaf(sv[4 * j + 2], kC, nm1)), p3 = ex2_approx(fmaf(sv[4 * j + 3], kC, nm1));
+          sum0 += p0 + p1;
+          sum1 += p2 + p3;
+          // the accumulator fragment of key tiles 2 kk, 2 kk + 1 is the A fragment of k-step kk
+          pa[j >> 1][(j & 1) * 2 + 0] = pack_bf16x2(p0, p1);
+          pa[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+        }
+        sum0 += __shfl_xor_sync(0xffffffffu, sum0, 1);
+        sum0 += __shfl_xor_sync(0xffffffffu, sum0, 2);
+        sum1 += __shfl_xor_sync(0xffffffffu, sum1, 1);
+        sum1 += __shfl_xor_sync(0xffffffffu, sum1, 2);
+        inv0 = 1.f / sum0;
+        inv1 = 1.f / sum1;
+      } else {
+#pragma unroll
+        for (int kk = 0; kk < kTok / 16; ++kk) pa[kk][0] = pa[kk][1] = pa[kk][2] = pa[kk][3] = 0u;
       }
-      tc_fence_before_sync();
+      // O = P V: wgmma is warpgroup-wide, the warps without real rows multiply zeros
+      float o[kHeadDim / 2];
+      wgmma_fence_regs(o);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kTok / 16; ++kk)
+        wgmma_rs_bt_n64(o, pa[kk], wgmma_desc_sw128(va + kk * 16 * kRowBytes), kk != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      if (active) {
+        // normalise, stage in this warp's own Q rows (read for the last time by S above), 128-byte coalesced scatter
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          *reinterpret_cast<uint32_t*>(stage + swz(qrow0, j) + t * 4) = pack_bf16x2(o[4 * j] * inv0, o[4 * j + 1] * inv0);
+          *reinterpret_cast<uint32_t*>(stage + swz(qrow1, j) + t * 4) = pack_bf16x2(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+        }
+        __syncwarp();
+        const long long row_base = static_cast<long long>(meta->batch[st]) * a.tokens_per_batch;
+        const int head = meta->head[st];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int row = row_w + i * 4 + (lane >> 3);
+          const int chunk = lane & 7;
+          const int src = meta->src[st][row];
+          if (src >= 0) {
+            const uint4 v = *reinterpret_cast<const uint4*>(stage + swz(row, chunk));
+            *reinterpret_cast<uint4*>(a.out + (row_base + src) * a.dim + head * kHeadDim + chunk * 8) = v;
+          }
+        }
+        fence_proxy_async_smem();  // the staged rows (generic proxy) are overwritten by the next TMA gather
+      }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&meta->p_full);
-      prev_src = my_src;
-      prev_inv = 1.f / sum;
-      prev_b = cur_b;
-      prev_head = cur_head;
+      if (lane == 0) mbar_arrive(&meta->empty[st]);  // q / k / v and the index map of this stage are consumed
     }
-    if (cnt > 0) epilogue(cnt - 1);
-  }
-
-  __syncwarp();
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -1047,7 +900,7 @@ extern "C" int ab_window_attention(const AbWindowAttention* p, void* stream) {
   a.num_heads = p->num_heads;
   a.dim = p->num_heads * kHeadDim;
   a.tokens_per_batch = static_cast<long long>(p->res[0]) * p->res[1] * p->res[2];
-  // Full 144-token windows (every production resolution) run on the tcgen05 / TMEM kernel.
+  // Full 144-token windows (every production resolution) run on the wgmma kernel.
   static const bool tc_disabled = getenv("AB_ATTN_NO_TC") != nullptr;
   if (!tc_disabled && a.g.ntok == tc::kTok && a.bias == nullptr) {
     static bool tc_attr_set = false;
@@ -1100,7 +953,7 @@ extern "C" int ab_window_attention(const AbWindowAttention* p, void* stream) {
     return AB_OK;
   }
   if (a.slab) {
-    set_error("ab_window_attention: latitude slabs need the tcgen05 kernel (AB_ATTN_NO_TC is set?)");
+    set_error("ab_window_attention: latitude slabs need the wgmma kernel (AB_ATTN_NO_TC is set?)");
     return AB_ERR_UNSUPPORTED;
   }
   const size_t smem = attn_smem_bytes(a.g.ntok);

@@ -1,9 +1,9 @@
-"""Forward engine: drives the sm_100a kernels of ``libaurora_b200.so`` through its C ABI.
+"""Forward engine: drives the sm_90a kernels of ``libaurora_b200.so`` through its C ABI.
 
 One ``AuroraEngine`` is bound to one set of parameters on one CUDA device.  PyTorch owns every buffer
 (weights, activations, workspace); all arithmetic on the per-step path happens inside the library:
 
-    Batch fields --ab_patchify--> bf16 token matrix --ab_gemm_bf16 (tcgen05)--> patch embeddings
+    Batch fields --ab_patchify--> bf16 token matrix --ab_gemm_bf16 (wgmma)--> patch embeddings
       -> Perceiver level aggregation (ab_gemm_bf16 / ab_perceiver_attention / ab_ln_mod_residual)
       -> 3-D Swin U-Net: per block  QKV GEMM -> ab_window_attention -> proj GEMM -> adaLN+residual
                                     -> fc1 GEMM(+GELU) -> fc2 GEMM -> adaLN+residual
@@ -111,15 +111,13 @@ class AuroraEngine:
         self.use_program = os.environ.get("AB_USE_PROGRAM", "1") != "0"
         self._programs: dict = {}
         # adaLN + residual fused into the epilogue of proj / fc2 (ab_gemm_ln_residual, D = 512 / 1024).  OFF by default:
-        # measured on B200 (profiles/r02_kernel_probes.md) the fused kernel is correct but 3 - 60 % SLOWER than the
-        # double-buffered GEMM followed by the row kernel, because a cluster that owns whole rows fills TMEM with one
-        # tile and cannot overlap its HBM-bound epilogue with the next main loop.  AB_FUSE_LN=1 turns it on.
+        # the fused kernel passes the same parity tests but has not been timed against GEMM + row kernel on H100 (its
+        # HBM-bound epilogue cannot overlap the next main loop of the same CTA).  AB_FUSE_LN=1 turns it on.
         self.fuse_ln = os.environ.get("AB_FUSE_LN", "0") == "1"
         # sharded forecast: the QKV projection's epilogue can store the boundary K | V rows into the neighbours' memory itself
-        # (fused compute + exchange, AbGemm.peer_push) instead of the copy kernel.  Bit-identical, but measured 4 % SLOWER
-        # per step at 4 GPUs (35.6 vs 34.2 ms, profiles/r02_kernel_probes.md): the epilogue's per-lane 16-byte stores make
-        # small NVLink packets and stall the epilogue warps, while the copy kernel keeps 2 CTAs per SM of wide stores in
-        # flight.  OFF by default; AB_FUSE_PUSH=1 turns it on.
+        # (fused compute + exchange, AbGemm.peer_push) instead of the copy kernel.  Bit-identical; not timed
+        # against the copy kernel (2 CTAs per SM of wide stores in flight) on NVLink-connected H100s.  OFF by default;
+        # AB_FUSE_PUSH=1 turns it on.
         self.fuse_push = os.environ.get("AB_FUSE_PUSH", "0") == "1"
         self._shard_plans = None
         # stage-level taps for parity tests: when set to a dict, `_run` stores fp32 copies of the encoder output and
@@ -134,7 +132,7 @@ class AuroraEngine:
         some = next(iter(params.values()))
         if not some.is_cuda:
             raise RuntimeError(
-                "aurora_b200 runs on CUDA devices only (sm_100a kernels); move the model with .to('cuda'). "
+                "aurora_b200 runs on CUDA devices only (sm_90a kernels); move the model with .to('cuda'). "
                 "There is no CPU fallback."
             )
         self.device = some.device

@@ -1,6 +1,6 @@
 """`Aurora` and its presets: same constructor arguments, ``state_dict`` keys, ``forward`` / checkpoint
 methods as the reference (`aurora/model/aurora.py:40-643`), with the forward pass executed by the
-sm_100a engine (``aurora_b200/engine.py``) instead of PyTorch modules.
+sm_90a engine (``aurora_b200/engine.py``) instead of PyTorch modules.
 
 The modules here are parameter containers only: they own fp32 ``nn.Parameter`` tensors under the
 reference's names so that ``load_state_dict`` / ``load_checkpoint_local`` accept the reference's
@@ -67,7 +67,7 @@ _SEAMS = {"backbone": _BackboneSeam, "encoder": _EncoderSeam}
 
 
 class Aurora(nn.Module):
-    """The Aurora model (1.3 B parameter configuration by default), running on B200 kernels.
+    """The Aurora model (1.3 B parameter configuration by default), running on H100 (sm_90a) kernels.
 
     Constructor arguments: see `aurora/model/aurora.py:55-178`; they are stored in ``self.config``.
     """
@@ -190,7 +190,7 @@ class Aurora(nn.Module):
         gets back ITS latitude band of the prediction (see `aurora_b200/sharding.py`; `gather_bands` rebuilds
         full fields)."""
         if not self.autocast:
-            # The reference's default (`autocast=False`, aurora.py:84) is a pure fp32 forward.  Blackwell has no fp32
+            # The reference's default (`autocast=False`, aurora.py:84) is a pure fp32 forward.  Hopper has no fp32
             # tensor-core path and this engine has no 3-pass split mode: it always computes with 16-bit operands and
             # fp32 accumulation, the reference's `autocast=True` recipe (aurora.py:327-343).  Running that under a
             # flag that promises fp32 would be a silent precision change, so it is refused.

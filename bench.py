@@ -2,18 +2,21 @@
 """Benchmark of the Aurora forward hot path (BASELINE.json: forecast-steps/sec on the 0.25-degree
 721x1440x13-level configuration, B = 1, history 2; 1.3 B-parameter `Aurora`).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
 
-* `--impl ours` (default): one "step" = one `Aurora.forward` through the sm_100a kernels.
+* `--impl ours` (default): one "step" = one `Aurora.forward` through the sm_90a kernels.
     value : steps/s with the input Batch already resident in HBM (CUDA events, max over ranks)
     e2e   : steps/s through the public API starting from PINNED HOST tensors, H2D of every input field
             and D2H of the whole prediction inside the timed region
-    roofline     : dominant kernel (tcgen05 GEMM): algorithmic FLOPs / CUDA-event time per launch vs the
-                   measured cuBLAS bf16 peak of MEASURED_PEAKS.json; plus the attention and adaLN kernels
+    roofline     : dominant kernel (wgmma GEMM): algorithmic FLOPs / CUDA-event time per launch vs the bf16 peak
+                   (MEASURED_PEAKS.json when present, else the H100 SXM data sheet); plus the attention and adaLN kernels
     cpu_baseline : the CPU oracle port timed on this box's host cores on a bounded sample (N = 1 only)
 * `--impl reference`: the reference algorithm's CPU implementation (oracle port; the Python reference
   itself cannot travel to the GPU box) on the host cores, each step a bounded sample extrapolated by
   algorithmic FLOPs.
+* `--dump-outputs DIR`: after the timed steps, the prediction of the LAST timed step is written to DIR as one float32
+  `<group>_<variable>.npy` per output field (a fixed, seeded sample of the points of a field when the whole prediction
+  would exceed 64 MB).  Inputs and weights are seeded, so two builds can be compared output for output.
 * N > 1: the forward pass does not need a collective for independent forecasts, so by default each rank runs
   its own replica of the workload ("weak" scaling, no data-path collective).  `--parallelism latshard` instead
   shards ONE forecast over the N GPUs by latitude band with an NCCL halo exchange per Swin block ("strong").
@@ -65,8 +68,8 @@ def peaks() -> dict:
         d = json.loads(f.read_text())
         return {"bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d["hbm_gbs"], "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": None, "hbm_gbs": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet (dense bf16, HBM3; a 700 W card), not a measurement"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -377,18 +380,23 @@ def _our_config(workload: str):
     return getattr(ab, WORKLOADS[workload][0])(_init="empty").config
 
 
-def gemm_traffic(workload: str, launches: int, algo_bytes: float) -> dict:
-    """`traffic` of the roofline object: DRAM bytes (read + write) per GEMM launch from the committed ncu pass
-    over one step of this workload (profiles/gemm_traffic.json, written by tools/ncu_traffic.py from the ncu CSV;
-    bench.py cannot run ncu itself), next to the compulsory bytes per launch counted from the launch arguments."""
-    out = {"traffic": None, "algorithmic_bytes": algo_bytes / launches if launches else None}
-    f = ROOT / "profiles" / "gemm_traffic.json"
-    if f.exists():
-        rec = json.loads(f.read_text()).get(workload)
-        if rec:
-            out["traffic"] = rec["dram_bytes_per_launch"]
-            out["traffic_source"] = rec["source"]
-    return out
+DUMP_BUDGET_BYTES = 64 * 2**20
+
+
+def dump_outputs(pred, out_dir: Path) -> None:
+    """The prediction as float32 `.npy` files, at most DUMP_BUDGET_BYTES in all: a field that does not fit its equal share
+    of the budget is sampled at seeded (hence run-to-run identical) flat indices."""
+    import numpy as np
+
+    fields = [(f"{grp}_{k}", v) for grp, d in (("surf", pred.surf_vars), ("atmos", pred.atmos_vars)) for k, v in d.items()]
+    share = DUMP_BUDGET_BYTES // (4 * len(fields)) - 64  # elements per field; 64: room for the .npy header
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for i, (name, v) in enumerate(fields):
+        flat = v.detach().reshape(-1)
+        if flat.numel() > share:
+            g = torch.Generator().manual_seed(1000 + i)
+            flat = flat[torch.randint(flat.numel(), (share,), generator=g).sort().values.to(flat.device)]
+        np.save(out_dir / f"{name}.npy", flat.float().cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -420,7 +428,7 @@ def workload_config(workload: str, gpus: int = 1, mode: str = "auto") -> dict:
             "history": 2, "algorithmic_tflop_per_step": ALGO_TFLOP[workload],
             "parallelism": {"single GPU": "single GPU", "replicas": f"replicas x{gpus} (one forecast per GPU)",
                             "latshard": f"one forecast latitude-sharded over {gpus} GPUs"}[par],
-            "l2": "inputs and activations are GBs per step (>> 126 MB L2): no explicit flush between iterations"}
+            "l2": "inputs and activations are GBs per step (>> 50 MB L2): no explicit flush between iterations"}
 
 
 def run_reference_arm(args) -> None:
@@ -471,6 +479,8 @@ def main() -> None:
                     help="also time one N-step autoregressive rollout (BASELINE configs[2]: 40) and add a `rollout` object")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", type=Path, default=None, metavar="DIR",
+                    help="write the prediction of the last timed step to DIR as float32 .npy files (<= 64 MB in all)")
     args = ap.parse_args()
     if args.warmup < 1:
         args.warmup = 1
@@ -540,6 +550,8 @@ def main() -> None:
     # kernels launched by this library in the timed region: eager launches + those replayed from captured graphs
     launches = (cabi.launch_count() - launches0) + (model._engine.replayed_launches - replayed0)
     ms = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(pred, args.dump_outputs)
 
     # ---- end to end through the public API from pinned host memory ----
     e2e_ms = None
@@ -631,11 +643,11 @@ def main() -> None:
     n_hw, t_hw, _, _ = agg("halo_wait")
     peak_tf = pk["bf16_tflops_sustained"] or pk["bf16_tflops"]
     roofline = {
-        "kernel": "gemm_bf16_tn_kernel (tcgen05)", "bound": "tensor",
+        "kernel": "gemm_bf16_tn_kernel (wgmma)", "bound": "tensor",
         "achieved": f_g / t_g / 1e12 if t_g else None, "peak": peak_tf, "unit": "TFLOP/s",
         "frac": (f_g / t_g / 1e12) / peak_tf if t_g else None,
-        **gemm_traffic(args.workload, n_g, b_g),
-        "peak_source": pk["source"] + " (sustained figure: kernel timed inside a long step)",
+        "algorithmic_bytes": b_g / n_g if n_g else None,
+        "peak_source": pk["source"],
         "launches_per_step": n_g, "seconds_per_step": t_g, "share_of_step": t_g / (ms / 1e3),
         "others": {
             "window_attention": {

@@ -1,5 +1,5 @@
 /*
- * aurora_b200.h — C ABI of libaurora_b200.so: the sm_100a kernels behind Aurora's forward pass.
+ * aurora_b200.h — C ABI of libaurora_b200.so: the sm_90a (Hopper) kernels behind Aurora's forward pass.
  *
  * The reference (microsoft/aurora) is pure Python/PyTorch and has no FFI; its seam is the Python
  * module boundary (Aurora.forward, aurora/model/aurora.py:265).  Every entry point below replaces a
@@ -52,8 +52,8 @@ unsigned long long ab_launch_count(void);
  *
  *   out[m, n] = act( sum_k A[m, k] * W[n, k] + bias[n] ) + residual[m, n]
  *
- * A: bf16|fp16 [M, K] (lda), W: same type [N, K] (ldw; nn.Linear layout), fp32 accumulation in TMEM
- * (tcgen05.mma kind::f16, TMA-staged 128B-swizzled operand tiles).  bias (f32 [N]) and residual
+ * A: bf16|fp16 [M, K] (lda), W: same type [N, K] (ldw; nn.Linear layout), fp32 accumulation in registers
+ * (wgmma.mma_async, TMA-staged 128B-swizzled operand tiles).  bias (f32 [N]) and residual
  * (f32 [M, ldr]) are optional (NULL).  act: AB_ACT_NONE or AB_ACT_GELU_ERF (exact erf GELU, as
  * nn.GELU()).  Either or both outputs may be requested: out_f32 [M, ld_f32], out_bf16 [M, ld_bf16].
  * Requirements: K % 8 == 0, lda % 8 == 0, ldw % 8 == 0, A/W 16-byte aligned.
@@ -62,7 +62,7 @@ enum { AB_ACT_NONE = 0, AB_ACT_GELU_ERF = 1 };
 
 /* 16-bit storage / tensor-core operand types.  The Swin backbone uses bf16 (the reference's autocast
  * recipe, aurora.py:327-343); encoder and decoder, which the reference keeps in fp32, use fp16 operands
- * (11-bit mantissa, same tcgen05 rate, saturating stores) to stay closer to it. */
+ * (11-bit mantissa, same wgmma rate, saturating stores) to stay closer to it. */
 enum { AB_DT_BF16 = 0, AB_DT_F16 = 1 };
 
 struct AbHaloPush; /* declared below */
@@ -281,7 +281,7 @@ int ab_swin_block(const AbSwinBlock* b, void* stream);
  *   out[m, :] = residual[m, :] + LN( A[m, :] · W^T + bias ) * scale + shift
  *
  * = ab_gemm_bf16 followed by ab_ln_mod_residual, in one kernel: the projection output never goes to HBM (the
- * statistics are taken on the fp32 accumulator in TMEM).  A cluster of CTA pairs owns whole rows, so N is fixed
+ * statistics are taken on the fp32 accumulator in registers).  A cluster of CTAs owns whole rows, so N is fixed
  * to 512 or 1024 (ab_gemm_ln_supported).  A, W: bf16|fp16 [M, K] / [N, K]; bias, scale, shift: f32 [N] or NULL
  * (0 / 1 / 0); residual f32 [M, ldr] or NULL; outputs f32 [M, ld_f32] (may alias residual) and / or 16-bit
  * [M, ld_16].  LN without affine, biased variance, eps as given.

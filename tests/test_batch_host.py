@@ -1,19 +1,21 @@
 """`Batch` / `Metadata` host logic (no GPU): validation and error behaviour of `aurora/batch.py:24-190`, the
-normalisation constants of `aurora/normalisation.py`, and — when the reference checkout is present (build
-container only) — a live cross-check of normalise / unnormalise / crop against the reference classes."""
+normalisation constants of `aurora/normalisation.py`, and a cross-check of normalise / unnormalise / crop / regrid
+against what the reference classes returned on the same inputs (stored by tests/golden/make_reference_golden.py)."""
 
-import sys
+import json
 from datetime import datetime
 from pathlib import Path
 
+import numpy as np
 import pytest
 import torch
 
 from aurora_b200 import Batch, Metadata
 from aurora_b200 import stats
 from tests import fixtures as fx
+from tests import reference_cases as rc
 
-REF = Path("/root/reference")
+GOLDEN = Path(__file__).parent / "golden"
 
 
 def _meta(h=17, w=32, **kw):
@@ -69,31 +71,20 @@ def test_normalise_roundtrip_and_overrides():
     assert stats.level_to_str(850) == "850" and stats.level_to_str(12.5) == "12_5"
 
 
-@pytest.mark.skipif(not REF.exists(), reason="reference checkout not present (GPU box)")
 def test_against_reference_classes_live():
-    sys.path[:0] = [str(REF), str(Path(__file__).parent / "_shims")]
-    try:
-        import aurora
-        from aurora import normalisation as rn
-    finally:
-        del sys.path[:2]
     # every normalisation constant of the reference is in our table, bit for bit as float64
-    assert stats.locations == {k: float(v) for k, v in rn.locations.items()}
-    assert stats.scales == {k: float(v) for k, v in rn.scales.items()}
-    cfg = fx.CONFIGS["tiny_air"]
-    b = fx.make_batch(cfg, 46, 90, levels=fx.LEVELS13, b=2)
-    rb = aurora.Batch(dict(b.surf_vars), dict(b.static_vars), dict(b.atmos_vars),
-                      aurora.Metadata(lat=b.metadata.lat, lon=b.metadata.lon, time=b.metadata.time,
-                                      atmos_levels=b.metadata.atmos_levels))
-    for ours, ref in ((b.normalise(), rb.normalise(surf_stats={})),
-                      (b.normalise().unnormalise(), rb.normalise(surf_stats={}).unnormalise(surf_stats={})),
-                      (b.crop(3), rb.crop(3))):
-        assert ours.spatial_shape == tuple(ref.spatial_shape)
+    ref_stats = json.loads((GOLDEN / "normalisation_ref.json").read_text())
+    assert stats.locations == ref_stats["locations"]
+    assert stats.scales == ref_stats["scales"]
+    b = rc.batch_case()
+    gold = np.load(GOLDEN / "batch_ref.npz")
+    for tag, ours in (("normalise", b.normalise()), ("roundtrip", b.normalise().unnormalise()), ("crop3", b.crop(3))):
+        assert ours.spatial_shape == tuple(gold[f"{tag}/shape"])
         for grp in ("surf_vars", "static_vars", "atmos_vars"):
-            assert list(getattr(ours, grp)) == list(getattr(ref, grp))
-            for k, v in getattr(ref, grp).items():
-                assert torch.equal(getattr(ours, grp)[k], v), (grp, k)
-        assert torch.equal(ours.metadata.lat, ref.metadata.lat)
+            assert list(getattr(ours, grp)) == list(gold[f"{tag}/{grp}"])
+            for k, v in getattr(ours, grp).items():
+                assert torch.equal(rc.sample(v), torch.from_numpy(gold[f"{tag}/{grp}/{k}"])), (grp, k)
+        assert torch.equal(ours.metadata.lat, torch.from_numpy(gold[f"{tag}/lat"]))
 
 
 def test_regrid_properties():
@@ -118,26 +109,21 @@ def test_regrid_properties():
     assert torch.allclose(fine.surf_vars["2t"][..., ::2, ::2], b.surf_vars["2t"], rtol=5e-6, atol=1e-4)
 
 
-@pytest.mark.skipif(not REF.exists(), reason="reference checkout not present (GPU box)")
-@pytest.mark.parametrize("res", [5.0, 11.25, 7.3])
+@pytest.mark.parametrize("res", rc.REGRID_RES)
 def test_regrid_against_reference_live(res):
-    sys.path[:0] = [str(REF), str(Path(__file__).parent / "_shims")]
-    try:
-        import aurora
-    finally:
-        del sys.path[:2]
-    cfg = fx.CONFIGS["tiny"]
-    b = fx.make_batch(cfg, 17, 32, levels=fx.LEVELS4, b=2)
-    rb = aurora.Batch(dict(b.surf_vars), dict(b.static_vars), dict(b.atmos_vars),
-                      aurora.Metadata(lat=b.metadata.lat, lon=b.metadata.lon, time=b.metadata.time,
-                                      atmos_levels=b.metadata.atmos_levels))
-    ours, ref = b.regrid(res), rb.regrid(res)
-    assert ours.spatial_shape == tuple(ref.spatial_shape)
-    assert torch.allclose(ours.metadata.lat, ref.metadata.lat, atol=1e-12) and torch.allclose(ours.metadata.lon, ref.metadata.lon, atol=1e-12)
+    gold = np.load(GOLDEN / "regrid_ref.npz")
+    ours = rc.regrid_case().regrid(res)
+    assert ours.spatial_shape == tuple(gold[f"{res}/shape"])
+    lat, lon = torch.from_numpy(gold[f"{res}/lat"]), torch.from_numpy(gold[f"{res}/lon"])
+    assert torch.allclose(ours.metadata.lat, lat, atol=1e-12) and torch.allclose(ours.metadata.lon, lon, atol=1e-12)
     for grp in ("surf_vars", "static_vars", "atmos_vars"):
-        for k, v in getattr(ref, grp).items():
+        assert list(getattr(ours, grp)) == list(gold[f"{res}/{grp}"])
+        for k in getattr(ours, grp):
+            v = torch.from_numpy(gold[f"{res}/{grp}/{k}"])
             got = getattr(ours, grp)[k]
-            assert got.dtype == torch.float32 and got.shape == v.shape
+            assert got.dtype == torch.float32 and rc.sample(got).shape == v.shape
+            assert got.shape[-2:] == ours.spatial_shape
+            got = rc.sample(got)
             assert torch.allclose(got, v, rtol=2e-6, atol=1e-6 * float(v.abs().max())), (grp, k, float((got - v).abs().max()))
 
 

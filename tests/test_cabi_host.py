@@ -1,4 +1,4 @@
-"""CPU-side checks of the C-ABI library: it builds for sm_100a, loads, exports every symbol that
+"""CPU-side checks of the C-ABI library: it builds for sm_90a, loads, exports every symbol that
 include/aurora_b200.h declares, validates arguments without touching a GPU, and its window index
 arithmetic (one __host__ __device__ routine shared with the attention kernel) is bit-exact against
 the reference-derived goldens."""

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (ab_gemm_bf16) against a plain PyTorch fp32 reference of the same op."""
+"""wgmma GEMM (ab_gemm_bf16) against a plain PyTorch fp32 reference of the same op."""
 
 import pytest
 import torch
@@ -30,9 +30,9 @@ SHAPES = [
     (4096, 2048, 512),   # fc1 stage-1-like, many tiles per CTA
     (2048, 512, 2048),   # fc2-like, long K
     (5, 16, 8),          # minimum sizes
-    # CTA-pair (cta_group::2) kernel: M >= 1024 and N >= 256
-    (1300, 520, 192),    # M tail inside the second CTA of a pair, N tail, 3 k-blocks
-    (2049, 256, 72),     # one row into a new pair (second CTA fully out of bounds), K tail
+    # many tiles, N = 256 blocks
+    (1300, 520, 192),    # M tail inside the second warpgroup's rows, N tail, 3 k-blocks
+    (2049, 256, 72),     # one row into a new tile (second warpgroup fully out of bounds), K tail
     (5000, 1536, 512),   # qkv-like, many tiles per cluster
     (1024, 300, 64),     # N tail in the only N block
 ]
@@ -64,10 +64,10 @@ def test_gemm_matches_fp32_reference(m, n, k, mode):
 
 
 WIDE_SHAPES = [
-    (1024, 256, 1024),    # two full 512-row cluster tiles
-    (1500, 520, 1024),    # M tail inside the second CTA's halves, N tail (8 live columns in the last block)
-    (2049, 256, 1088),    # one row into a new tile (three of four 128-row boxes fully out of bounds), odd k-block count
-    (20000, 1536, 1024),  # several tiles per cluster: accumulator hand-over between tiles
+    (1024, 256, 1024),    # eight full 128-row tiles
+    (1500, 520, 1024),    # M tail inside the second warpgroup's rows, N tail (8 live columns in the last block)
+    (2049, 256, 1088),    # one row into a new tile (all but one 16-row box fully out of bounds), odd k-block count
+    (20000, 1536, 1024),  # several tiles per CTA: the accumulator registers are reused between tiles
     (4096, 512, 4096),    # long K
 ]
 
@@ -75,8 +75,9 @@ WIDE_SHAPES = [
 @pytest.mark.parametrize("m,n,k", WIDE_SHAPES)
 @pytest.mark.parametrize("mode", ["plain_bf16", "bias_gelu_bf16", "bias_res_f32_dual"])
 def test_wide_pair_kernel_matches_reference_and_pair_kernel(m, n, k, mode, monkeypatch):
-    """512 x 256 cluster-tile kernel (AB_GEMM_WIDE=2 forces it): fp32 reference tolerance, and bit-identical to
-    the 256 x 256 pair kernel (same fp32 accumulation order over K)."""
+    """Large shapes with K >= 1024 (long main loops, many tiles per CTA): fp32 reference tolerance, and two launches on
+    the same operands are bit-identical (the persistent schedule fixes the fp32 accumulation order over K).  The name
+    dates from a kernel family that had a separate wide-tile variant for these shapes."""
     from aurora_b200 import cabi
 
     torch.manual_seed(m + n + k)
@@ -87,8 +88,7 @@ def test_wide_pair_kernel_matches_reference_and_pair_kernel(m, n, k, mode, monke
     residual = torch.randn(m, n, device=dev) if mode == "bias_res_f32_dual" else None
     act = cabi.AB_ACT_GELU_ERF if mode == "bias_gelu_bf16" else cabi.AB_ACT_NONE
     outs = {}
-    for wide in ("2", "0"):
-        monkeypatch.setenv("AB_GEMM_WIDE", wide)
+    for wide in ("2", "0"):  # first and second launch
         out_bf16 = torch.full((m, n), float("nan"), device=dev, dtype=torch.bfloat16)
         out_f32 = torch.full((m, n), float("nan"), device=dev) if mode == "bias_res_f32_dual" else None
         cabi.gemm(a, w, bias=bias, residual=residual, out_f32=out_f32, out_bf16=out_bf16, act=act)
@@ -135,12 +135,12 @@ def test_gemm_rejects_bad_arguments():
 # projection with adaLN + residual fused into the epilogue (csrc/gemm_ln.cu)
 # ------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("m,n,k", [
-    (1000, 512, 512),     # proj-like, M tail inside the second CTA of the pair
+    (1000, 512, 512),     # proj-like, M tail inside the last tile
     (5000, 512, 2048),    # fc2-like, many tiles per cluster, long K
     (37, 512, 128),       # fewer rows than one CTA holds
-    (785, 1024, 1024),    # two CTA pairs per cluster: row statistics meet through distributed shared memory
+    (785, 1024, 1024),    # four CTAs per cluster: row statistics meet through distributed shared memory
     (20000, 1024, 4096),  # stage-2 fc2-like
-    (300, 1024, 72),      # K tail (K % 64 != 0), P = 2
+    (300, 1024, 72),      # K tail (K % 64 != 0), cluster of 4
 ])
 @pytest.mark.parametrize("mode", ["inplace_bf16", "f16_wide_ld", "no_residual_f32_only"])
 def test_gemm_ln_residual_matches_fp32_reference(m, n, k, mode):
@@ -203,14 +203,14 @@ def test_gemm_epilogue_pushes_boundary_rows_into_halo_slots(variant, to_above, t
     """The QKV projection of a latitude band [C, rows, W, 3D] with `peer_push`: columns [D, 3D) of the first `to_above`
     and last `to_below` rows of every level land in the halo slots (here: in this GPU's own memory) exactly as
     `ab_halo_push` would place them, the round is published in both flags once, the completion counter is back at zero,
-    and the regular output is untouched by the extra stores.  All three GEMM kernels (single CTA, CTA pair, wide pair)."""
+    and the regular output is untouched by the extra stores.  "single": fewer tiles than SMs; "pair" / "wide": the
+    full-size band, several tiles per CTA (the names date from a kernel family with one variant per size class)."""
     from aurora_b200 import cabi
 
     c, rows, w, d, k, slot_rows = 4, 10, 36, 256, 1024, 5
     if variant == "single":
-        rows, w = 5, 12          # M = 240 < 1024: single-CTA kernel
+        rows, w = 5, 12          # M = 240: two row tiles
         to_above, to_below = min(to_above, rows), min(to_below, rows)
-    monkeypatch.setenv("AB_GEMM_WIDE", "2" if variant == "wide" else "0")
     m, n = c * rows * w, 3 * d
     torch.manual_seed(c + rows + w + to_above)
     dev = "cuda"

@@ -1,4 +1,4 @@
-"""End-to-end parity of the CUDA path: `aurora_b200.Aurora*.forward` / `rollout` on a B200 against
+"""End-to-end parity of the CUDA path: `aurora_b200.Aurora*.forward` / `rollout` on an H100 against
 (a) golden outputs of the unmodified reference (tests/golden/model_*.npz, float64 reference) and
 (b) the CPU oracle run live on the same seeded inputs.
 
@@ -159,7 +159,7 @@ def test_sharded_step_replays_from_graph_segments():
     eagerly between them.  On one GPU (world size 1) the band is the whole grid and the halo wraps onto itself, so
     the segmented replay must reproduce the eager sharded step and the plain forward bit for bit."""
     cfg, model = _build("tiny_lora", "Aurora", 17)
-    # patch_res (4, 48, 64): full 144-token windows at all three stages (the tcgen05 slab kernel)
+    # patch_res (4, 48, 64): full 144-token windows at all three stages (the wgmma slab kernel)
     b1 = fx.make_batch(cfg, 192, 256, levels=fx.LEVELS4, b=1, seed=17, rollout_step=1)
     b2 = fx.make_batch(cfg, 192, 256, levels=fx.LEVELS4, b=1, seed=18, rollout_step=1)
     plain = {k: v.clone() for k, v in model.forward(b1).atmos_vars.items()}
