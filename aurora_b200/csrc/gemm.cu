@@ -4,14 +4,21 @@
 //
 //   warpgroup 0    : TMA producer (one lane) — 128B-swizzled {64 x 128} A tiles and {64 x BN} W tiles into a ring of
 //                    shared-memory stages; gives its registers up (setmaxnreg) to the math warpgroups
-//   warpgroups 1-2 : math + epilogue — each owns 64 of the tile's 128 rows: wgmma.mma_async m64nBNk16 straight from the
-//                    swizzled stages, the 64 x BN fp32 accumulator in registers; bias / erf-GELU / residual on the
-//                    registers, 16-bit-only outputs through swizzled shared memory and a TMA store
+//   warpgroups 1-2 : math + epilogue — wgmma.mma_async m64nBNk16 straight from the swizzled stages into fp32
+//                    register accumulators; bias / erf-GELU / residual on the registers, 16-bit-only outputs through
+//                    two alternating swizzled shared-memory boxes per warp and TMA stores
 //
 // Pipelines: full / empty mbarriers per stage (TMA <-> wgmma) and the static persistent tile schedule
 // (tile = blockIdx.x + i * gridDim.x, N-blocks fastest so that the CTAs running concurrently share the same A rows in
-// L2 while W stays L2-resident).  One wgmma group stays in flight while the next stage is waited for; while the math
-// warpgroups run a tile's epilogue the producer already fills the ring with the next tile's operands.
+// L2 while W stays L2-resident), loaded by the producer in order.  Two ways to share it (see the kernel):
+//   cooperative : both math warpgroups work on every 128 x BN tile, 64 rows each (BN = 64 / 128 / 256)
+//   ping-pong   : warpgroup w takes the positions i = w, w + 2, ... and all 128 rows of each 128 x 128 tile (two
+//                 m64n128k16 per k16 sharing the W descriptor); it starts a main loop only once the other has issued
+//                 the last k-block of its previous tile (two "order" mbarriers), so that one warpgroup's epilogue runs
+//                 while the other's wgmmas keep the tensor pipe busy
+// ab_gemm_bf16 takes ping-pong where the epilogue is a large part of a tile's time (K <= 1024, N > 128) and the
+// cooperative tile elsewhere, whose wgmmas read fewer shared-memory bytes per FLOP.  One wgmma group stays in flight
+// while the next stage is waited for.
 //
 // Replaces: every nn.Linear on Aurora's forward path (see include/aurora_b200.h).
 #include <stdlib.h>
@@ -26,9 +33,10 @@ namespace ab {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 bytes = one swizzle row
 constexpr int kWgmmaK = 16;
-constexpr int kMathWarps = 8;  // two warpgroups x 64 rows
+constexpr int kMathWarps = 8;  // two warpgroups, one tile each
 constexpr int kNumThreads = 128 + kMathWarps * 32;
-constexpr int kBoxRows = 16;   // rows of one epilogue box = rows of the accumulator one warp holds
+constexpr int kBoxRows = 16;   // rows of one epilogue box = rows of one m64 accumulator that one warp holds
+constexpr int kBoxBytes = kBoxRows * 128;
 
 template <int BN>
 struct GemmCfg {
@@ -37,9 +45,9 @@ struct GemmCfg {
   static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
   static constexpr int kStages = BN >= 256 ? 4 : (BN >= 128 ? 6 : 8);
   static constexpr int kBarrierBytes = 256;
-  static constexpr int kStagingBytes = kMathWarps * kBoxRows * 128;  // one 16-row x 128-byte store box per math warp
+  static constexpr int kStagingBytes = kMathWarps * 2 * kBoxBytes;  // two 16-row x 128-byte store boxes per math warp
   static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBarrierBytes + 1024;  // +1024: alignment
-  static_assert(2 * kStages * 8 <= kBarrierBytes, "barrier area");
+  static_assert((2 * kStages + 2) * 8 <= kBarrierBytes, "barrier area");
   static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 };
 
@@ -119,102 +127,137 @@ __device__ __forceinline__ void bias_act2(const GemmArgs& g, int col, float& x0,
 
 // General epilogue: this thread's two rows (row0, row0 + 8) x BN / 4 columns of the accumulator straight to global
 // memory.  A quad of lanes covers 8 consecutive columns: 32 bytes of the fp32 output, 16 bytes of the 16-bit one.
+// Row-major order keeps one row's addresses live at a time (the register budget is set by the accumulators).
 template <int BN>
 __device__ __forceinline__ void epilogue_direct(const GemmArgs& g, float (&acc)[BN / 2], int row0, int col0) {
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int col = col0 + 8 * j;
-    if (col >= g.n) continue;
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + 8 * h;
+    if (row >= g.m) continue;
+    const float* const res = g.residual + static_cast<size_t>(row) * g.ldr;
+    float* const o32 = g.out_f32 + static_cast<size_t>(row) * g.ld_f32;
+    uint16_t* const o16 = g.out_bf16 + static_cast<size_t>(row) * g.ld_bf16;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = row0 + 8 * h;
-      if (row >= g.m) continue;
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = col0 + 8 * j;
+      if (col >= g.n) continue;
       float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
       bias_act2(g, col, x0, x1);
       if (g.vec_ok && col + 1 < g.n) {
         if (g.residual != nullptr) {
-          const float2 r = __ldg(reinterpret_cast<const float2*>(g.residual + static_cast<size_t>(row) * g.ldr + col));
+          const float2 r = __ldg(reinterpret_cast<const float2*>(res + col));
           x0 += r.x;
           x1 += r.y;
         }
-        if (g.out_f32 != nullptr)
-          *reinterpret_cast<float2*>(g.out_f32 + static_cast<size_t>(row) * g.ld_f32 + col) = make_float2(x0, x1);
+        if (g.out_f32 != nullptr) *reinterpret_cast<float2*>(o32 + col) = make_float2(x0, x1);
         if (g.out_bf16 != nullptr)
-          *reinterpret_cast<uint32_t*>(g.out_bf16 + static_cast<size_t>(row) * g.ld_bf16 + col) =
-              g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
+          *reinterpret_cast<uint32_t*>(o16 + col) = g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
       } else {
         const float x[2] = {x0, x1};
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           if (col + e >= g.n) continue;
           float v = x[e];
-          if (g.residual != nullptr) v += __ldg(g.residual + static_cast<size_t>(row) * g.ldr + col + e);
-          if (g.out_f32 != nullptr) g.out_f32[static_cast<size_t>(row) * g.ld_f32 + col + e] = v;
-          if (g.out_bf16 != nullptr) g.out_bf16[static_cast<size_t>(row) * g.ld_bf16 + col + e] = to16(v, g.out_half);
+          if (g.residual != nullptr) v += __ldg(res + col + e);
+          if (g.out_f32 != nullptr) o32[col + e] = v;
+          if (g.out_bf16 != nullptr) o16[col + e] = to16(v, g.out_half);
         }
       }
     }
   }
 }
 
-// 16-bit-only epilogue: per 64-column box, bias / activation on the registers, 16-bit pairs into this warp's staging
-// box (16 rows x 128 bytes, 128B swizzle: chunk ^= row & 7, the layout a CU_TENSOR_MAP_SWIZZLE_128B store expects;
-// the 8 rows x 4 lanes of one store instruction hit 32 different banks), then one asynchronous TMA store: full
-// 128-byte rows, M / N tails clipped by the tensor map.  Rows that a neighbouring GPU needs are copied out of the
-// staging box into its halo slot, 16 bytes per lane.
+// 16-bit-only epilogue of one 16-row x 64-column box (rows row0 .. row0 + 15 of the output, columns colb ..): bias /
+// activation on the registers, 16-bit pairs into one of this warp's two staging boxes (16 rows x 128 bytes, 128B
+// swizzle: chunk ^= row & 7, the layout a CU_TENSOR_MAP_SWIZZLE_128B store expects; the 8 rows x 4 lanes of one store
+// instruction hit 32 different banks), then one asynchronous TMA store: full 128-byte rows, M / N tails clipped by the
+// tensor map.  The two buffers alternate per issued store, so filling one only waits for the store issued two boxes
+// ago.  Rows that a neighbouring GPU needs are copied out of the staging box into its halo slot, 16 bytes per lane.
 template <int BN>
-__device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmap_out, float (&acc)[BN / 2],
-                                             uint8_t* stage, int warp_row0, int n0, int lane) {
+__device__ __forceinline__ void epilogue_tma_box(const GemmArgs& g, const CUtensorMap* tmap_out, const float (&acc)[BN / 2],
+                                                 int c, uint8_t* staging, uint32_t& nst, int row0, int colb,
+                                                 int lane) {
+  if (row0 >= g.m) return;  // warp-uniform: the box lies below the matrix
+  uint8_t* const stage = staging + (nst & 1u) * kBoxBytes;
   const int r = lane >> 2, t = lane & 3;
   const uint32_t st0 = smem_u32(stage) + r * 128 + t * 4;
+  if (lane == 0) tma_store_wait_read<1>();  // the store that last read this buffer is done with it
+  __syncwarp();
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+    const int j = 8 * c + jj;
+    float x0 = acc[4 * j], x1 = acc[4 * j + 1], y0 = acc[4 * j + 2], y1 = acc[4 * j + 3];
+    if (g.bias != nullptr) {  // one load for both rows; columns past N get 0 (the tensor map clips them)
+      const int col = colb + 8 * jj + 2 * t;
+      float2 b = make_float2(0.f, 0.f);
+      if (col + 1 < g.n) b = __ldg(reinterpret_cast<const float2*>(g.bias + col));
+      else if (col < g.n) b.x = __ldg(g.bias + col);
+      x0 += b.x;
+      x1 += b.y;
+      y0 += b.x;
+      y1 += b.y;
+    }
+    if (g.act == AB_ACT_GELU_ERF) {
+      x0 = gelu_erf(x0);
+      x1 = gelu_erf(x1);
+      y0 = gelu_erf(y0);
+      y1 = gelu_erf(y1);
+    }
+    const uint32_t off = static_cast<uint32_t>((jj ^ (r & 7)) << 4);
+    const uint32_t lo = g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
+    const uint32_t hi = g.out_half ? pack_f16x2(y0, y1) : pack_bf16x2(y0, y1);
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + off), "r"(lo) : "memory");
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + 8 * 128 + off), "r"(hi) : "memory");
+  }
+  if (g.peer.n_ranges > 0) {
+    __syncwarp();
+    bool any = false;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int lr = 4 * i + (lane >> 3), chunk = lane & 7;
+      uint16_t* const dst = peer_row_ptr(g, row0 + lr, colb);
+      if (dst != nullptr) {
+        any = true;
+        *reinterpret_cast<uint4*>(dst + chunk * 8) =
+            *reinterpret_cast<const uint4*>(stage + lr * 128 + ((chunk ^ (lr & 7)) << 4));
+      }
+    }
+    if (__any_sync(0xffffffffu, any)) peer_box_done(g, lane);
+  }
+  fence_proxy_async_smem();
+  __syncwarp();
+  if (lane == 0) {
+    tma_store_2d(tmap_out, stage, colb, row0);
+    tma_store_commit();
+  }
+  ++nst;
+}
+
+// 16-bit-only epilogue of a warpgroup's kRB x 64 rows: per 64-column box, each 64-row block in turn.
+template <int BN, int kRB>
+__device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmap_out, const float (&acc)[kRB][BN / 2],
+                                             uint8_t* staging, uint32_t& nst, int warp_row0, int n0, int lane) {
 #pragma unroll
   for (int c = 0; c < BN / 64; ++c) {
     const int colb = n0 + 64 * c;
     if (colb >= g.n) continue;  // warp-uniform
-    if (lane == 0) tma_store_wait_read<0>();  // the previous box of this warp has left the staging buffer
-    __syncwarp();
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      const int j = 8 * c + jj;
-      const int col = colb + 8 * jj + 2 * t;
-      float x0 = acc[4 * j], x1 = acc[4 * j + 1], y0 = acc[4 * j + 2], y1 = acc[4 * j + 3];
-      bias_act2(g, col, x0, x1);
-      bias_act2(g, col, y0, y1);
-      const uint32_t off = static_cast<uint32_t>((jj ^ (r & 7)) << 4);
-      const uint32_t lo = g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
-      const uint32_t hi = g.out_half ? pack_f16x2(y0, y1) : pack_bf16x2(y0, y1);
-      asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + off), "r"(lo) : "memory");
-      asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + 8 * 128 + off), "r"(hi) : "memory");
-    }
-    if (g.peer.n_ranges > 0) {
-      __syncwarp();
-      bool any = false;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int lr = 4 * i + (lane >> 3), chunk = lane & 7;
-        uint16_t* const dst = peer_row_ptr(g, warp_row0 + lr, colb);
-        if (dst != nullptr) {
-          any = true;
-          *reinterpret_cast<uint4*>(dst + chunk * 8) =
-              *reinterpret_cast<const uint4*>(stage + lr * 128 + ((chunk ^ (lr & 7)) << 4));
-        }
-      }
-      if (__any_sync(0xffffffffu, any)) peer_box_done(g, lane);
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0 && warp_row0 < g.m) {
-      tma_store_2d(tmap_out, stage, colb, warp_row0);
-      tma_store_commit();
-    }
+    for (int rb = 0; rb < kRB; ++rb)
+      epilogue_tma_box<BN>(g, tmap_out, acc[rb], c, staging, nst, warp_row0 + 64 * rb, colb, lane);
   }
 }
 
-template <int BN, bool kHalfIn>
+// kPingPong = false, "cooperative": both math warpgroups work on every tile of the CTA, warpgroup w on rows
+//   [64 w, 64 w + 64) (one m64nBNk16 accumulator each, BN up to 256).
+// kPingPong = true: warpgroup w takes the tiles at positions w, w + 2, ... of the CTA's sequence and all 128 rows of
+//   each (two m64nBNk16 accumulators, BN = 128); it starts a main loop only once the other warpgroup has issued the
+//   last k-block of the tile before, so that one warpgroup's epilogue runs under the other's wgmmas.
+template <int BN, bool kPingPong, bool kHalfIn>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_out, const GemmArgs g) {
   using Cfg = GemmCfg<BN>;
+  constexpr int kRB = kPingPong ? 2 : 1;  // 64-row accumulator blocks per warpgroup
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte alignment.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -223,6 +266,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   uint8_t* smem_stage_out = smem + Cfg::kStages * Cfg::kStageBytes;  // 1024-byte aligned (stages are)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
+  uint64_t* order_bar = empty_bar + Cfg::kStages;  // ping-pong, [w]: math warpgroup w may start its next main loop
 
   const int warp = threadIdx.x >> 5;  // warp-uniform
   const int lane = threadIdx.x & 31;
@@ -233,8 +277,10 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     if (g.tma_out) prefetch_tmap(&tmap_out);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kMathWarps);
+      mbar_init(&empty_bar[s], kPingPong ? 4 : kMathWarps);  // the warps that consume the stage
     }
+    mbar_init(&order_bar[0], 4);
+    mbar_init(&order_bar[1], 4);
     fence_mbar_init();
   }
   __syncthreads();
@@ -263,29 +309,43 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
       }
     }
   } else {
-    // ===== math warpgroups: rows [64 wg, 64 wg + 64) of the tile =====
+    // ===== math warpgroups =====
     reg_alloc<232>();
     const int wg = (warp >> 2) - 1;
-    const int warp_row = wg * 64 + (warp & 3) * kBoxRows;  // first of this warp's 16 accumulator rows inside the tile
-    uint8_t* const stage = smem_stage_out + (warp - 4) * (kBoxRows * 128);
-    float acc[BN / 2];
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    // first of this warp's 16 rows inside the tile (inside each 64-row block for ping-pong)
+    const int warp_row = (kPingPong ? 0 : wg * 64) + (warp & 3) * kBoxRows;
+    uint8_t* const staging = smem_stage_out + (warp - 4) * (2 * kBoxBytes);
+    float acc[kRB][BN / 2];
+    uint32_t nst = 0;  // TMA stores this warp has issued: picks the staging buffer
+    constexpr int kStep = kPingPong ? 2 : 1;
+    uint32_t j = 0;  // tiles this warpgroup has taken
+    for (int i = kPingPong ? wg : 0;; i += kStep, ++j) {
+      const int tile = blockIdx.x + i * gridDim.x;
+      if (tile >= num_tiles) break;
       const int m0 = (tile / num_n) * kBlockM;
       const int n0 = (tile % num_n) * BN;
+      // ping-pong: tile i - 1 (the other warpgroup's) has issued all its wgmmas
+      if (kPingPong && i > 0) mbar_wait(&order_bar[wg], (wg == 0 ? j - 1 : j) & 1u);
+      uint32_t it = static_cast<uint32_t>(i) * num_kb;  // the ring position of this tile's first k-block
       int prev_s = -1;
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const uint32_t s = it % Cfg::kStages;
         mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1u);
-        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + wg * (64 * 128);
+        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + (kPingPong ? 0 : wg * (64 * 128));
         const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
-        wgmma_fence_regs(acc);
+#pragma unroll
+        for (int rb = 0; rb < kRB; ++rb) wgmma_fence_regs(acc[rb]);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
-          wgmma_ss<BN, kHalfIn>(acc, wgmma_desc_sw128(a_addr + k * kWgmmaK * 2), wgmma_desc_sw128(b_addr + k * kWgmmaK * 2),
-                                (kb | k) != 0 ? 1u : 0u);
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+          const uint64_t desc_b = wgmma_desc_sw128(b_addr + k * kWgmmaK * 2);
+#pragma unroll
+          for (int rb = 0; rb < kRB; ++rb)
+            wgmma_ss<BN, kHalfIn>(acc[rb], wgmma_desc_sw128(a_addr + rb * (64 * 128) + k * kWgmmaK * 2), desc_b,
+                                  (kb | k) != 0 ? 1u : 0u);
+        }
         wgmma_commit();
+        if (kPingPong && kb == num_kb - 1 && lane == 0) mbar_arrive(&order_bar[wg ^ 1]);  // hand the tensor pipe over
         if (prev_s >= 0) {
           wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand its shared memory back to the producer
           if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
@@ -293,16 +353,22 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         prev_s = static_cast<int>(s);
       }
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+#pragma unroll
+      for (int rb = 0; rb < kRB; ++rb) wgmma_fence_regs(acc[rb]);
       if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
-      if (g.tma_out) epilogue_tma<BN>(g, &tmap_out, acc, stage, m0 + warp_row, n0, lane);
-      else epilogue_direct<BN>(g, acc, m0 + warp_row + (lane >> 2), n0 + 2 * (lane & 3));
+      if (g.tma_out) {
+        epilogue_tma<BN, kRB>(g, &tmap_out, acc, staging, nst, m0 + warp_row, n0, lane);
+      } else {
+#pragma unroll
+        for (int rb = 0; rb < kRB; ++rb)
+          epilogue_direct<BN>(g, acc[rb], m0 + 64 * rb + warp_row + (lane >> 2), n0 + 2 * (lane & 3));
+      }
     }
     if (g.tma_out && lane == 0) tma_store_wait_all<0>();  // smem must outlive the bulk stores
   }
 }
 
-template <int BN, bool kHalfIn>
+template <int BN, bool kPingPong, bool kHalfIn>
 static int launch_gemm(const AbGemm* p, const GemmArgs& args, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   CUtensorMap ta, tw;
@@ -317,8 +383,8 @@ static int launch_gemm(const AbGemm* p, const GemmArgs& args, cudaStream_t strea
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, kHalfIn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, kPingPong, kHalfIn>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("ab_gemm_bf16: cudaFuncSetAttribute(smem=%d) failed: %s", Cfg::kSmemBytes, cudaGetErrorString(e));
       return AB_ERR_CUDA;
@@ -327,7 +393,7 @@ static int launch_gemm(const AbGemm* p, const GemmArgs& args, cudaStream_t strea
   }
   const long long tiles = ceil_div_ll(p->m, kBlockM) * ceil_div_ll(p->n, BN);
   const int grid = static_cast<int>(tiles < sm_count() ? tiles : sm_count());
-  gemm_bf16_tn_kernel<BN, kHalfIn><<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
+  gemm_bf16_tn_kernel<BN, kPingPong, kHalfIn><<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
   AB_COUNT_LAUNCH(1);
   AB_CHECK_LAUNCH("ab_gemm_bf16");
   return AB_OK;
@@ -430,12 +496,19 @@ extern "C" int ab_gemm_bf16(const AbGemm* p, void* stream) {
     pr.expected = groups * ((p->n - pr.col_from + 63) / 64);
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  // Ping-pong for K <= 1024 and N > 128: there the epilogue is a large part of a tile's time and runs hidden under the
+  // other warpgroup's main loop.  From K = 2048 on the cooperative 128 x 256 tile is as fast or faster: its wgmmas read
+  // fewer shared-memory bytes per FLOP (B once for 128 rows, 48 KB of operands per 128 x 256 x 64 step against 32 KB
+  // per 128 x 128 x 64), and the main loop dominates.  The decoder heads (N = 80 and 64) stay cooperative as well.
+  const bool ping_pong = p->n > 128 && p->k <= 1024;
   if (p->in_dtype == AB_DT_F16) {
-    if (p->n > 128) return launch_gemm<256, true>(p, a, s);
-    if (p->n > 64) return launch_gemm<128, true>(p, a, s);
-    return launch_gemm<64, true>(p, a, s);
+    if (ping_pong) return launch_gemm<128, true, true>(p, a, s);
+    if (p->n > 128) return launch_gemm<256, false, true>(p, a, s);
+    if (p->n > 64) return launch_gemm<128, false, true>(p, a, s);
+    return launch_gemm<64, false, true>(p, a, s);
   }
-  if (p->n > 128) return launch_gemm<256, false>(p, a, s);
-  if (p->n > 64) return launch_gemm<128, false>(p, a, s);
-  return launch_gemm<64, false>(p, a, s);
+  if (ping_pong) return launch_gemm<128, true, false>(p, a, s);
+  if (p->n > 128) return launch_gemm<256, false, false>(p, a, s);
+  if (p->n > 64) return launch_gemm<128, false, false>(p, a, s);
+  return launch_gemm<64, false, false>(p, a, s);
 }
