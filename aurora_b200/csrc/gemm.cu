@@ -6,7 +6,8 @@
 //                    shared-memory stages; gives its registers up (setmaxnreg) to the math warpgroups
 //   warpgroups 1-2 : math + epilogue — wgmma.mma_async m64nBNk16 straight from the swizzled stages into fp32
 //                    register accumulators; bias / erf-GELU / residual on the registers, 16-bit-only outputs through
-//                    two alternating swizzled shared-memory boxes per warp and TMA stores
+//                    two alternating swizzled shared-memory boxes per warp and TMA stores, with the tile's bias
+//                    copied into shared memory when the tile starts
 //
 // Pipelines: full / empty mbarriers per stage (TMA <-> wgmma) and the static persistent tile schedule
 // (tile = blockIdx.x + i * gridDim.x, N-blocks fastest so that the CTAs running concurrently share the same A rows in
@@ -19,6 +20,10 @@
 // ab_gemm_bf16 takes ping-pong where the epilogue is a large part of a tile's time (K <= 1024, N > 128) and the
 // cooperative tile elsewhere, whose wgmmas read fewer shared-memory bytes per FLOP.  One wgmma group stays in flight
 // while the next stage is waited for.
+//
+// Phase trace: built with -DAB_GEMM_TRACE (tools/gemm_trace.py does that into build/trace/), the kernel sums
+// clock64() cycles per warp role and phase in registers and writes them once per CTA into a device buffer set with
+// ab_gemm_trace(); without the switch the trace code compiles to nothing.
 //
 // Replaces: every nn.Linear on Aurora's forward path (see include/aurora_b200.h).
 #include <stdlib.h>
@@ -38,7 +43,7 @@ constexpr int kNumThreads = 128 + kMathWarps * 32;
 constexpr int kBoxRows = 16;   // rows of one epilogue box = rows of one m64 accumulator that one warp holds
 constexpr int kBoxBytes = kBoxRows * 128;
 
-template <int BN>
+template <int BN, bool kPingPong>
 struct GemmCfg {
   static constexpr int kStageBytesA = kBlockM * kBlockK * 2;
   static constexpr int kStageBytesB = BN * kBlockK * 2;
@@ -46,9 +51,46 @@ struct GemmCfg {
   static constexpr int kStages = BN >= 256 ? 4 : (BN >= 128 ? 6 : 8);
   static constexpr int kBarrierBytes = 256;
   static constexpr int kStagingBytes = kMathWarps * 2 * kBoxBytes;  // two 16-row x 128-byte store boxes per math warp
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBarrierBytes + 1024;  // +1024: alignment
+  // the tile's BN bias values: one copy per warpgroup for ping-pong (each has its own tile), one for cooperative
+  static constexpr int kBiasGroups = kPingPong ? 2 : 1;
+  static constexpr int kBiasThreads = kMathWarps * 32 / kBiasGroups;  // the math threads that share a copy
+  static constexpr int kBiasBytes = kBiasGroups * BN * 4;
+  static constexpr int kSmemBytes =
+      kStages * kStageBytes + kStagingBytes + kBiasBytes + kBarrierBytes + 1024;  // +1024: alignment
   static_assert((2 * kStages + 2) * 8 <= kBarrierBytes, "barrier area");
   static_assert(kSmemBytes <= 227 * 1024, "shared memory");
+};
+
+// Phase trace slots (see Trace).  A CTA's record is kTrCta 64-bit words, then kTrSlots per math warp.
+enum TraceCta { kTrTimerStart, kTrTimerEnd, kTrClockStart, kTrClockEnd, kTrEmptyWait, kTrProducerTiles, kTrCta };
+enum TraceSlot {
+  kTrFullFirst,  // full_bar wait of a tile's first k-block (producer: empty_bar waits)
+  kTrFullRest,   // full_bar waits of its other k-blocks
+  kTrOrder,      // order_bar wait (ping-pong)
+  kTrWait1,      // wgmma_wait<1> in the main loop
+  kTrWait0,      // wgmma_wait<0> after it
+  kTrEpi,        // the whole epilogue
+  kTrEpiStore,   // of which: waits for a store buffer
+  kTrEpiBias,    // of which: waits for the bias values
+  kTrTiles,      // tiles taken
+  kTrSlots
+};
+#ifdef AB_GEMM_TRACE
+constexpr int kTrWords = kTrCta + kMathWarps * kTrSlots;
+#endif
+
+// Per-thread cycle sums of the phase trace; without AB_GEMM_TRACE every member is empty and compiles away.
+struct Trace {
+#ifdef AB_GEMM_TRACE
+  uint32_t c[kTrSlots] = {};
+  __device__ __forceinline__ long long now() const { return clock64(); }
+  __device__ __forceinline__ void add(int slot, long long t0) { c[slot] += static_cast<uint32_t>(clock64() - t0); }
+  __device__ __forceinline__ void tick(int slot) { ++c[slot]; }
+#else
+  __device__ __forceinline__ long long now() const { return 0; }
+  __device__ __forceinline__ void add(int, long long) {}
+  __device__ __forceinline__ void tick(int) {}
+#endif
 };
 
 // Rows of the 16-bit output that are ALSO stored into a neighbouring GPU's memory by the epilogue (the K | V halo rows of
@@ -75,8 +117,11 @@ struct GemmArgs {
   int act;
   int vec_ok;    // all leading dimensions / pointers allow 16-byte vector access
   int out_half;  // 16-bit output is fp16 instead of bf16
-  int tma_out;   // 16-bit-only output written through swizzled smem + TMA store (tmap_out valid)
+  int tma_out;   // 16-bit-only output written through swizzled smem + TMA store (tmap_out valid), bias staged in smem
   PeerRows peer;
+#ifdef AB_GEMM_TRACE
+  unsigned long long* trace;  // kTrWords per CTA
+#endif
 };
 
 // Destination in a neighbour's memory of columns col .. col + 64 of output row `row`, or nullptr.
@@ -167,47 +212,78 @@ __device__ __forceinline__ void epilogue_direct(const GemmArgs& g, float (&acc)[
   }
 }
 
-// 16-bit-only epilogue of one 16-row x 64-column box (rows row0 .. row0 + 15 of the output, columns colb ..): bias /
-// activation on the registers, 16-bit pairs into one of this warp's two staging boxes (16 rows x 128 bytes, 128B
-// swizzle: chunk ^= row & 7, the layout a CU_TENSOR_MAP_SWIZZLE_128B store expects; the 8 rows x 4 lanes of one store
-// instruction hit 32 different banks), then one asynchronous TMA store: full 128-byte rows, M / N tails clipped by the
-// tensor map.  The two buffers alternate per issued store, so filling one only waits for the store issued two boxes
-// ago.  Rows that a neighbouring GPU needs are copied out of the staging box into its halo slot, 16 bytes per lane.
+// Copy of the tile's bias values n0 .. n0 + BN into the group's shared-memory slice, asynchronously (cp.async, 16 bytes
+// per thread, waited for at the epilogue); columns past N read 0.  Issued at the start of a tile so that the epilogue
+// has no global load: a bias __ldg there waits on L2 once per box.  kThreads: the math threads that share the slice.
+template <int BN, int kThreads>
+__device__ __forceinline__ void stage_bias(const GemmArgs& g, float* bias_s, int n0, int tid) {
+  static_assert(BN / 4 <= kThreads, "one 16-byte copy per thread");
+  if (tid < BN / 4) {
+    const int col = n0 + 4 * tid;
+    const int bytes = col >= g.n ? 0 : (g.n - col >= 4 ? 16 : 4 * (g.n - col));
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(bias_s + 4 * tid)),
+                 "l"(g.bias + (bytes > 0 ? col : 0)), "r"(bytes)
+                 : "memory");
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// Named barrier of the kThreads math threads that share a bias slice (id 0 is __syncthreads).
+template <int kThreads>
+__device__ __forceinline__ void group_sync(int id) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(kThreads) : "memory");
+}
+
+// 16-bit-only epilogue of one 16-row x 64-column box (rows row0 .. row0 + 15 of the output, columns colb ..): bias (from
+// the group's shared-memory copy) / activation on the registers, 16-bit pairs into one of this warp's two staging boxes
+// (16 rows x 128 bytes, 128B swizzle: chunk ^= row & 7, the layout a CU_TENSOR_MAP_SWIZZLE_128B store expects), then
+// one asynchronous TMA store: full 128-byte rows, M / N tails clipped by the tensor map.  The staging stores are
+// stmatrix, 4 per box where 32-bit stores would take 16: in ping-pong they queue for shared memory behind the other
+// warpgroup's wgmma operand reads, and fewer of them shorten the epilogue (4.8 against 5.0 µs per tile, stage-1 qkv).  The two buffers alternate per issued
+// store, so filling one only waits for the store issued two boxes ago.  Rows that a neighbouring GPU needs are copied
+// out of the staging box into its halo slot, 16 bytes per lane.
 template <int BN>
 __device__ __forceinline__ void epilogue_tma_box(const GemmArgs& g, const CUtensorMap* tmap_out, const float (&acc)[BN / 2],
-                                                 int c, uint8_t* staging, uint32_t& nst, int row0, int colb,
-                                                 int lane) {
+                                                 const float* bias_s, int c, uint8_t* staging, uint32_t& nst,
+                                                 int row0, int colb, int lane, Trace& tr) {
   if (row0 >= g.m) return;  // warp-uniform: the box lies below the matrix
   uint8_t* const stage = staging + (nst & 1u) * kBoxBytes;
-  const int r = lane >> 2, t = lane & 3;
-  const uint32_t st0 = smem_u32(stage) + r * 128 + t * 4;
+  const int t = lane & 3;
+  const long long t0 = tr.now();
   if (lane == 0) tma_store_wait_read<1>();  // the store that last read this buffer is done with it
   __syncwarp();
+  tr.add(kTrEpiStore, t0);
+  // stmatrix: four 8 x 8 16-bit matrices per instruction, (jj, rows 0-7), (jj, rows 8-15), (jj + 1, rows 0-7),
+  // (jj + 1, rows 8-15), in the accumulator's fragment layout; lane l gives the address of row l & 7 of matrix l >> 3
+  const int mi = lane >> 3, rr = lane & 7;
+  const uint32_t row_addr = smem_u32(stage) + (rr + 8 * (mi & 1)) * 128;
 #pragma unroll
-  for (int jj = 0; jj < 8; ++jj) {
-    const int j = 8 * c + jj;
-    float x0 = acc[4 * j], x1 = acc[4 * j + 1], y0 = acc[4 * j + 2], y1 = acc[4 * j + 3];
-    if (g.bias != nullptr) {  // one load for both rows; columns past N get 0 (the tensor map clips them)
-      const int col = colb + 8 * jj + 2 * t;
-      float2 b = make_float2(0.f, 0.f);
-      if (col + 1 < g.n) b = __ldg(reinterpret_cast<const float2*>(g.bias + col));
-      else if (col < g.n) b.x = __ldg(g.bias + col);
-      x0 += b.x;
-      x1 += b.y;
-      y0 += b.x;
-      y1 += b.y;
+  for (int jj = 0; jj < 8; jj += 2) {
+    uint32_t v[4];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int j = 8 * c + jj + q;
+      float x0 = acc[4 * j], x1 = acc[4 * j + 1], y0 = acc[4 * j + 2], y1 = acc[4 * j + 3];
+      if (g.bias != nullptr) {  // one load for both rows; columns past N hold 0 (the tensor map clips them)
+        const float2 b = *reinterpret_cast<const float2*>(bias_s + 8 * j + 2 * t);
+        x0 += b.x;
+        x1 += b.y;
+        y0 += b.x;
+        y1 += b.y;
+      }
+      if (g.act == AB_ACT_GELU_ERF) {
+        x0 = gelu_erf(x0);
+        x1 = gelu_erf(x1);
+        y0 = gelu_erf(y0);
+        y1 = gelu_erf(y1);
+      }
+      v[2 * q] = g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
+      v[2 * q + 1] = g.out_half ? pack_f16x2(y0, y1) : pack_bf16x2(y0, y1);
     }
-    if (g.act == AB_ACT_GELU_ERF) {
-      x0 = gelu_erf(x0);
-      x1 = gelu_erf(x1);
-      y0 = gelu_erf(y0);
-      y1 = gelu_erf(y1);
-    }
-    const uint32_t off = static_cast<uint32_t>((jj ^ (r & 7)) << 4);
-    const uint32_t lo = g.out_half ? pack_f16x2(x0, x1) : pack_bf16x2(x0, x1);
-    const uint32_t hi = g.out_half ? pack_f16x2(y0, y1) : pack_bf16x2(y0, y1);
-    asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + off), "r"(lo) : "memory");
-    asm volatile("st.shared.b32 [%0], %1;" ::"r"(st0 + 8 * 128 + off), "r"(hi) : "memory");
+    const uint32_t addr = row_addr + (((jj + (mi >> 1)) ^ rr) << 4);
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]),
+                 "r"(v[2]), "r"(v[3])
+                 : "memory");
   }
   if (g.peer.n_ranges > 0) {
     __syncwarp();
@@ -236,14 +312,15 @@ __device__ __forceinline__ void epilogue_tma_box(const GemmArgs& g, const CUtens
 // 16-bit-only epilogue of a warpgroup's kRB x 64 rows: per 64-column box, each 64-row block in turn.
 template <int BN, int kRB>
 __device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmap_out, const float (&acc)[kRB][BN / 2],
-                                             uint8_t* staging, uint32_t& nst, int warp_row0, int n0, int lane) {
+                                             const float* bias_s, uint8_t* staging, uint32_t& nst, int warp_row0,
+                                             int n0, int lane, Trace& tr) {
 #pragma unroll
   for (int c = 0; c < BN / 64; ++c) {
     const int colb = n0 + 64 * c;
     if (colb >= g.n) continue;  // warp-uniform
 #pragma unroll
     for (int rb = 0; rb < kRB; ++rb)
-      epilogue_tma_box<BN>(g, tmap_out, acc[rb], c, staging, nst, warp_row0 + 64 * rb, colb, lane);
+      epilogue_tma_box<BN>(g, tmap_out, acc[rb], bias_s, c, staging, nst, warp_row0 + 64 * rb, colb, lane, tr);
   }
 }
 
@@ -256,7 +333,7 @@ template <int BN, bool kPingPong, bool kHalfIn>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_out, const GemmArgs g) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, kPingPong>;
   constexpr int kRB = kPingPong ? 2 : 1;  // 64-row accumulator blocks per warpgroup
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte alignment.
@@ -264,12 +341,21 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kStageBytesA;
   uint8_t* smem_stage_out = smem + Cfg::kStages * Cfg::kStageBytes;  // 1024-byte aligned (stages are)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes);
+  float* smem_bias = reinterpret_cast<float*>(smem_stage_out + Cfg::kStagingBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes + Cfg::kBiasBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
   uint64_t* order_bar = empty_bar + Cfg::kStages;  // ping-pong, [w]: math warpgroup w may start its next main loop
 
   const int warp = threadIdx.x >> 5;  // warp-uniform
   const int lane = threadIdx.x & 31;
+  Trace tr;
+#ifdef AB_GEMM_TRACE
+  unsigned long long* const trace = g.trace + static_cast<size_t>(blockIdx.x) * kTrWords;
+  if (threadIdx.x == 0) {
+    trace[kTrTimerStart] = global_timer_ns();
+    trace[kTrClockStart] = clock64();
+  }
+#endif
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
@@ -301,12 +387,19 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const uint32_t s = it % Cfg::kStages;
           const uint32_t ph = (it / Cfg::kStages) & 1u;
+          const long long t0 = tr.now();
           mbar_wait(&empty_bar[s], ph ^ 1u);
+          tr.add(kTrFullFirst, t0);
           mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
           tma_load_2d(smem_a + s * Cfg::kStageBytesA, &tmap_a, &full_bar[s], kb * kBlockK, m0);
           tma_load_2d(smem_b + s * Cfg::kStageBytesB, &tmap_w, &full_bar[s], kb * kBlockK, n0);
         }
+        tr.tick(kTrTiles);
       }
+#ifdef AB_GEMM_TRACE
+      trace[kTrEmptyWait] = tr.c[kTrFullFirst];
+      trace[kTrProducerTiles] = tr.c[kTrTiles];
+#endif
     }
   } else {
     // ===== math warpgroups =====
@@ -315,6 +408,10 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     // first of this warp's 16 rows inside the tile (inside each 64-row block for ping-pong)
     const int warp_row = (kPingPong ? 0 : wg * 64) + (warp & 3) * kBoxRows;
     uint8_t* const staging = smem_stage_out + (warp - 4) * (2 * kBoxBytes);
+    // the bias copy of this warp's group (ping-pong: its warpgroup; cooperative: both) and the group's named barrier
+    const int bias_group = kPingPong ? wg : 0;
+    float* const bias_s = smem_bias + bias_group * BN;
+    const int bias_tid = threadIdx.x - 128 - bias_group * Cfg::kBiasThreads;
     float acc[kRB][BN / 2];
     uint32_t nst = 0;  // TMA stores this warp has issued: picks the staging buffer
     constexpr int kStep = kPingPong ? 2 : 1;
@@ -324,13 +421,24 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
       if (tile >= num_tiles) break;
       const int m0 = (tile / num_n) * kBlockM;
       const int n0 = (tile % num_n) * BN;
+      if (g.tma_out && g.bias != nullptr) {
+        group_sync<Cfg::kBiasThreads>(1 + bias_group);  // the group's previous epilogue has read the old values
+        stage_bias<BN, Cfg::kBiasThreads>(g, bias_s, n0, bias_tid);
+      }
       // ping-pong: tile i - 1 (the other warpgroup's) has issued all its wgmmas
-      if (kPingPong && i > 0) mbar_wait(&order_bar[wg], (wg == 0 ? j - 1 : j) & 1u);
+      if (kPingPong && i > 0) {
+        const long long t0 = tr.now();
+        mbar_wait(&order_bar[wg], (wg == 0 ? j - 1 : j) & 1u);
+        tr.add(kTrOrder, t0);
+      }
       uint32_t it = static_cast<uint32_t>(i) * num_kb;  // the ring position of this tile's first k-block
       int prev_s = -1;
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const uint32_t s = it % Cfg::kStages;
+        const long long t0 = tr.now();
         mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1u);
+        if (kb == 0) tr.add(kTrFullFirst, t0);
+        else tr.add(kTrFullRest, t0);
         const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + (kPingPong ? 0 : wg * (64 * 128));
         const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
 #pragma unroll
@@ -347,30 +455,58 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         wgmma_commit();
         if (kPingPong && kb == num_kb - 1 && lane == 0) mbar_arrive(&order_bar[wg ^ 1]);  // hand the tensor pipe over
         if (prev_s >= 0) {
+          const long long t1 = tr.now();
           wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand its shared memory back to the producer
+          tr.add(kTrWait1, t1);
           if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
         }
         prev_s = static_cast<int>(s);
       }
+      long long t0 = tr.now();
       wgmma_wait<0>();
 #pragma unroll
       for (int rb = 0; rb < kRB; ++rb) wgmma_fence_regs(acc[rb]);
+      tr.add(kTrWait0, t0);
       if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
+      t0 = tr.now();
       if (g.tma_out) {
-        epilogue_tma<BN, kRB>(g, &tmap_out, acc, staging, nst, m0 + warp_row, n0, lane);
+        if (g.bias != nullptr) {
+          const long long t1 = tr.now();
+          asm volatile("cp.async.wait_all;" ::: "memory");
+          group_sync<Cfg::kBiasThreads>(1 + bias_group);  // every thread's copy has landed
+          tr.add(kTrEpiBias, t1);
+        }
+        epilogue_tma<BN, kRB>(g, &tmap_out, acc, bias_s, staging, nst, m0 + warp_row, n0, lane, tr);
       } else {
 #pragma unroll
         for (int rb = 0; rb < kRB; ++rb)
           epilogue_direct<BN>(g, acc[rb], m0 + 64 * rb + warp_row + (lane >> 2), n0 + 2 * (lane & 3));
       }
+      tr.add(kTrEpi, t0);
+      tr.tick(kTrTiles);
     }
     if (g.tma_out && lane == 0) tma_store_wait_all<0>();  // smem must outlive the bulk stores
+#ifdef AB_GEMM_TRACE
+    if (lane == 0)
+      for (int s = 0; s < kTrSlots; ++s) trace[kTrCta + (warp - 4) * kTrSlots + s] = tr.c[s];
+#endif
   }
+#ifdef AB_GEMM_TRACE
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    trace[kTrClockEnd] = clock64();
+    trace[kTrTimerEnd] = global_timer_ns();
+  }
+#endif
 }
 
+#ifdef AB_GEMM_TRACE
+static unsigned long long* g_trace_buf = nullptr;
+#endif
+
 template <int BN, bool kPingPong, bool kHalfIn>
-static int launch_gemm(const AbGemm* p, const GemmArgs& args, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+static int launch_gemm(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN, kPingPong>;
   CUtensorMap ta, tw;
   int rc = make_tmap_16bit_2d(&ta, p->a, p->m, p->k, p->lda, kBlockM, kBlockK, kHalfIn);
   if (rc != AB_OK) return rc;
@@ -393,11 +529,24 @@ static int launch_gemm(const AbGemm* p, const GemmArgs& args, cudaStream_t strea
   }
   const long long tiles = ceil_div_ll(p->m, kBlockM) * ceil_div_ll(p->n, BN);
   const int grid = static_cast<int>(tiles < sm_count() ? tiles : sm_count());
+#ifdef AB_GEMM_TRACE
+  AB_CHECK_ARG(g_trace_buf != nullptr, "ab_gemm_bf16: traced build without a trace buffer (ab_gemm_trace)");
+  args.trace = g_trace_buf;
+#endif
   gemm_bf16_tn_kernel<BN, kPingPong, kHalfIn><<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
   AB_COUNT_LAUNCH(1);
   AB_CHECK_LAUNCH("ab_gemm_bf16");
   return AB_OK;
 }
+
+#ifdef AB_GEMM_TRACE
+// Traced builds only: every later launch writes its phase record (kTrWords 64-bit words per CTA, at most one CTA per
+// SM) into buf.  Returns kTrWords.
+extern "C" int ab_gemm_trace(unsigned long long* buf) {
+  ab::g_trace_buf = buf;
+  return ab::kTrWords;
+}
+#endif
 
 }  // namespace ab
 
@@ -437,7 +586,7 @@ extern "C" int ab_gemm_bf16(const AbGemm* p, void* stream) {
              (p->out_bf16 == nullptr || p->ld_bf16 % 8 == 0);
 
   memset(&a.peer, 0, sizeof(a.peer));
-  // TMA-store epilogue: 16-bit output only, no residual, 16-byte aligned rows.
+  // TMA-store epilogue: 16-bit output only, no residual, 16-byte aligned rows and bias.
   a.tma_out = p->out_bf16 != nullptr && p->out_f32 == nullptr && p->residual == nullptr && al16(p->out_bf16) &&
               p->ld_bf16 % 8 == 0 && (p->bias == nullptr || (reinterpret_cast<uintptr_t>(p->bias) & 15u) == 0);
   if (p->peer_push != nullptr) {
