@@ -19,7 +19,7 @@ __all__ = [
     "window_index_map", "ln_mod_residual", "patch_merge_ln", "patch_split_ln", "perceiver_attention",
     "linear_small", "patchify", "unpatchify", "AbFieldIn", "AbFieldOut", "ipc_export", "ipc_open", "ipc_close",
     "halo_push", "halo_wait", "AbSwinBlock", "swin_block", "swin_block_workspace_bytes", "gemm_ln_supported",
-    "gemm_ln_residual",
+    "gemm_ln_residual", "AbTrackBox", "track_boxes",
 ]
 
 ABI_VERSION = 2  # == AB_ABI_VERSION in include/aurora_b200.h
@@ -116,6 +116,7 @@ EXPORTS = [
     "ab_gemm_ln_residual",
     "ab_run_ops",
     "ab_struct_size",
+    "ab_track_boxes",
 ]
 AB_IPC_HANDLE_BYTES = 64
 AB_HALO_CTRL_BYTES = 256
@@ -671,3 +672,30 @@ def make_program(recorded: list):
 
 def run_ops(program) -> None:
     check(lib().ab_run_ops(program, len(program), _s()), "ab_run_ops")
+
+
+# ---- tropical-cyclone tracking boxes (csrc/tracker.cu) ------------------------------------------------------------
+AB_TRACK_MINIMA, AB_TRACK_MAX, AB_TRACK_MIN, AB_TRACK_WINDMAX = 0, 1, 2, 3
+AB_TRACK_MAX_SIDE = 101
+AB_TRACK_MAX_BOXES = 32
+
+
+class AbTrackBox(C.Structure):
+    _fields_ = [
+        ("plane", C.c_void_p), ("plane2", C.c_void_p),
+        ("h", C.c_int32), ("w", C.c_int32), ("ld", C.c_int32), ("op", C.c_int32),
+        ("rows_off", C.c_int32), ("n_rows", C.c_int32), ("cols_off", C.c_int32), ("n_cols", C.c_int32),
+        ("mask_off", C.c_int64),
+    ]
+
+
+def track_boxes(boxes: list, index: torch.Tensor, values: torch.Tensor, counts: torch.Tensor,
+                masks: Optional[torch.Tensor]) -> None:
+    """One launch over `boxes` (`AbTrackBox` list); `index` int32, `values` f32 and `counts` int32 [len(boxes)],
+    `masks` uint8, all on the device."""
+    assert index.dtype == torch.int32 and values.dtype == torch.float32 and counts.dtype == torch.int32
+    assert values.numel() >= len(boxes) and counts.numel() >= len(boxes)
+    arr = (AbTrackBox * len(boxes))(*boxes)
+    check(lib().ab_track_boxes(arr, len(boxes), C.c_size_t(C.sizeof(AbTrackBox)), C.c_void_p(ptr(index)),
+                               C.c_void_p(ptr(values)), C.c_void_p(ptr(counts)), C.c_void_p(ptr(masks)), _s()),
+          "ab_track_boxes")

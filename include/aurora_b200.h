@@ -425,6 +425,43 @@ typedef struct AbOp {
 
 int ab_run_ops(const AbOp* ops, int32_t n_ops, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Tropical-cyclone tracking on device-resident predictions (the reference's aurora/tracker.py:61-104,
+ * 185-196, 262-282): ONE launch evaluates
+ * a list of boxes, one CTA per box, and writes a few bytes per box; the scalar decisions stay with the caller.  A box
+ * is the cross product of a row-index list and a column-index list into one field plane (lists, because the
+ * reference's longitude selection wraps around and concatenates two ranges, :36-47).
+ *
+ *   AB_TRACK_MINIMA   masks[mask_off ..] = uint8 [n_rows, n_cols] row-major: the local minima of the box after
+ *                     scipy.ndimage.gaussian_filter(box, sigma=1) (radius 4, float64 accumulation, rounded to f32 per
+ *                     axis) and an 8 x 8 minimum filter, both with mode "reflect"; border rows / columns cleared.
+ *                     counts[i] = number of minima.
+ *   AB_TRACK_MAX      values[i] = max of the box                 (the land test `lsm_box.max() < 0.5`)
+ *   AB_TRACK_MIN      values[i] = min of the box                 (minimum msl of the crop)
+ *   AB_TRACK_WINDMAX  values[i] = max of sqrt(u*u + v*v), u = plane, v = plane2, each operation rounded as numpy
+ *                     float32 does
+ * Reductions propagate NaN like numpy.  The index lists are DEVICE int32 memory (`index`); every entry is checked
+ * against the plane's extent in the kernel, and a box with an entry outside it gets counts[i] = -1 and values[i] = NaN.
+ * `boxes` is a HOST array; `box_bytes` must be sizeof(AbTrackBox).  1 <= n_rows, n_cols <= AB_TRACK_MAX_SIDE and
+ * n_boxes <= AB_TRACK_MAX_BOXES (the descriptors travel as kernel parameters); larger boxes are AB_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+enum { AB_TRACK_MINIMA = 0, AB_TRACK_MAX = 1, AB_TRACK_MIN = 2, AB_TRACK_WINDMAX = 3 };
+#define AB_TRACK_MAX_SIDE 101 /* delta 5 at 0.1 degrees, the finest grid of the shipped models */
+#define AB_TRACK_MAX_BOXES 32
+
+typedef struct AbTrackBox {
+  const float* plane;  /* f32 [h, ld] */
+  const float* plane2; /* AB_TRACK_WINDMAX: the v plane, same layout as `plane`; NULL otherwise */
+  int32_t h, w, ld;    /* extent of the plane and elements between its rows */
+  int32_t op;          /* AB_TRACK_* */
+  int32_t rows_off, n_rows; /* row indices: index[rows_off .. rows_off + n_rows) */
+  int32_t cols_off, n_cols; /* column indices: index[cols_off .. cols_off + n_cols) */
+  int64_t mask_off;    /* AB_TRACK_MINIMA: byte offset of the box's mask in `masks` */
+} AbTrackBox;
+
+int ab_track_boxes(const AbTrackBox* boxes, int32_t n_boxes, size_t box_bytes, const int32_t* index, float* values,
+                   int32_t* counts, uint8_t* masks, void* stream);
+
 /* sizeof() of the descriptor structs as this library was compiled (binding authors: compare with your mirror).
  * which: 0 AbGemm, 1 AbWindowAttention, 2 AbLnModResidual, 3 AbFieldIn, 4 AbFieldOut, 5 AbHaloPush, 6 AbSwinBlock,
  * 7 AbGemmLn, 8 AbPatchMergeLn, 9 AbPatchSplitLn, 10 AbOp; -1 for an unknown index.  Host only. */
