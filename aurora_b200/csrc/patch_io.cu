@@ -41,13 +41,14 @@ __device__ __forceinline__ float transform_in(const AbFieldIn& f, float x) {
       default: return nan_to_num0(cosf(v * kDegToRad));
     }
   }
-  if (f.transform >= 1) v = fmaxf(v, 0.f);
+  // the clamps keep NaN as torch.clamp does (fmaxf would turn it into the bound)
+  if (f.transform >= 1) v = fmax_keep_nan(v, 0.f);
   if (f.transform == 2) {
     // AuroraAirPollution._pre_encoder_hook: Linear(2,1)([clamp(z,0,2.5), (log(max(z,eps)) - log eps) / -log eps])
     const float eps = 1e-4f;
     const float ln_eps = -9.210340371976182f;
-    const float a0 = fminf(fmaxf(v, 0.f), 2.5f);
-    const float a1 = (logf(fmaxf(v, eps)) - ln_eps) / (-ln_eps);
+    const float a0 = fmin_keep_nan(fmax_keep_nan(v, 0.f), 2.5f);
+    const float a1 = (logf(fmax_keep_nan(v, eps)) - ln_eps) / (-ln_eps);
     v = f.w0 * a0 + f.w1 * a1 + f.wb;
   }
   return v;
@@ -130,8 +131,8 @@ __global__ void __launch_bounds__(256) unpatchify_kernel(const __grid_constant__
       const float prev = (__ldg(f.prev + pix + p2) - f.loc) / f.scale;
       val = val + (1.f + mod) * prev;
     }
-    if (f.clamp_max1) val = fminf(val, 1.f);
-    if (f.clamp_min0) val = fmaxf(val, 0.f);
+    if (f.clamp_max1) val = fmin_keep_nan(val, 1.f);  // NaN stays NaN, as with torch.clamp
+    if (f.clamp_min0) val = fmax_keep_nan(val, 0.f);
     if (f.dens_col >= 0) {
       // density = sigmoid(logit) * wmb_mask; data = value * wmb_mask; data[density < 0.5] = NaN (aurora.py:906-918)
       const float m = __ldg(f.mask + pix + p2) > f.mask_min ? 1.f : 0.f;

@@ -175,12 +175,24 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// Round to nearest fp16 with finite overflow and +-inf saturated to +-65504 (fp16 overflows where bf16 would not);
+// NaN stays NaN.  One F2FP.SATFINITE instruction for the pair.
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
-  // saturating conversion: fp16 overflows at 65504 where bf16 would not
-  lo = fminf(fmaxf(lo, -65504.f), 65504.f);
-  hi = fminf(fmaxf(hi, -65504.f), 65504.f);
-  __half2 v = __floats2half2_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&v);
+  uint32_t u;
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(u) : "f"(hi), "f"(lo));
+  return u;
+}
+
+// fmaxf / fminf return the other operand when one is NaN; these return NaN, as torch.clamp does.
+__device__ __forceinline__ float fmax_keep_nan(float a, float b) {
+  float d;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+__device__ __forceinline__ float fmin_keep_nan(float a, float b) {
+  float d;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
 }
 
 // 16-bit storage types selected at run time: 0 = bf16 (the backbone, as the reference's autocast),
@@ -213,10 +225,7 @@ __device__ __forceinline__ uint4 pack16x8(const float (&f)[8]) {
   return u;
 }
 __device__ __forceinline__ uint16_t to16(float x, int half) {
-  if (half) {
-    __half h = __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f));
-    return *reinterpret_cast<uint16_t*>(&h);
-  }
+  if (half) return static_cast<uint16_t>(pack_f16x2(x, 0.f));
   __nv_bfloat16 b = __float2bfloat16_rn(x);
   return *reinterpret_cast<uint16_t*>(&b);
 }
