@@ -19,7 +19,7 @@ __all__ = [
     "window_index_map", "ln_mod_residual", "patch_merge_ln", "patch_split_ln", "perceiver_attention",
     "linear_small", "patchify", "unpatchify", "AbFieldIn", "AbFieldOut", "ipc_export", "ipc_open", "ipc_close",
     "halo_push", "halo_wait", "AbSwinBlock", "swin_block", "swin_block_workspace_bytes", "gemm_ln_supported",
-    "gemm_ln_residual", "AbTrackBox", "track_boxes",
+    "gemm_ln_residual", "AbTrackBox", "track_boxes", "AbScoreField", "score_workspace_bytes", "score_fields",
 ]
 
 ABI_VERSION = 2  # == AB_ABI_VERSION in include/aurora_b200.h
@@ -117,6 +117,8 @@ EXPORTS = [
     "ab_run_ops",
     "ab_struct_size",
     "ab_track_boxes",
+    "ab_score_workspace_bytes",
+    "ab_score_fields",
 ]
 AB_IPC_HANDLE_BYTES = 64
 AB_HALO_CTRL_BYTES = 256
@@ -699,3 +701,37 @@ def track_boxes(boxes: list, index: torch.Tensor, values: torch.Tensor, counts: 
     check(lib().ab_track_boxes(arr, len(boxes), C.c_size_t(C.sizeof(AbTrackBox)), C.c_void_p(ptr(index)),
                                C.c_void_p(ptr(values)), C.c_void_p(ptr(counts)), C.c_void_p(ptr(masks)), _s()),
           "ab_track_boxes")
+
+
+# ---- latitude-weighted scores (csrc/score.cu) ---------------------------------------------------------------------
+AB_SCORE_MAX_FIELDS = 64
+AB_SCORE_SUMS = 8  # W, sum w d, sum w d^2, sum w |d|, sum w af ao, sum w af^2, sum w ao^2, count
+
+
+class AbScoreField(C.Structure):
+    _fields_ = [
+        ("pred", C.c_void_p), ("truth", C.c_void_p), ("clim", C.c_void_p),
+        ("pred_level_stride", C.c_int64), ("truth_level_stride", C.c_int64), ("clim_level_stride", C.c_int64),
+        ("h", C.c_int32), ("w", C.c_int32),
+        ("ld_pred", C.c_int32), ("ld_truth", C.c_int32), ("ld_clim", C.c_int32),
+        ("levels", C.c_int32),
+    ]
+
+
+def score_workspace_bytes(fields: list) -> int:
+    arr = (AbScoreField * max(len(fields), 1))(*fields)
+    n = C.c_size_t()
+    check(lib().ab_score_workspace_bytes(arr, len(fields), C.c_size_t(C.sizeof(AbScoreField)), C.byref(n)),
+          "ab_score_workspace_bytes")
+    return int(n.value)
+
+
+def score_fields(fields: list, row_weights: torch.Tensor, sums: torch.Tensor, workspace: torch.Tensor) -> None:
+    """One call over `fields` (`AbScoreField` list): `row_weights` float64 [h], `sums` float64 [planes, 8] (a view with
+    contiguous rows), `workspace` of at least `score_workspace_bytes(fields)` bytes, all on the device."""
+    assert row_weights.dtype == torch.float64 and sums.dtype == torch.float64 and sums.is_contiguous()
+    arr = (AbScoreField * max(len(fields), 1))(*fields)
+    nbytes = workspace.numel() * workspace.element_size()
+    check(lib().ab_score_fields(arr, len(fields), C.c_size_t(C.sizeof(AbScoreField)), C.c_void_p(ptr(row_weights)),
+                                C.c_void_p(ptr(sums)), C.c_void_p(ptr(workspace)), C.c_size_t(nbytes), _s()),
+          "ab_score_fields")

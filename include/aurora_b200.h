@@ -462,6 +462,42 @@ typedef struct AbTrackBox {
 int ab_track_boxes(const AbTrackBox* boxes, int32_t n_boxes, size_t box_bytes, const int32_t* index, float* values,
                    int32_t* counts, uint8_t* masks, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Latitude-weighted scores of device-resident predictions against a truth (and a climatology): the sums behind
+ * RMSE, bias, MAE and the uncentred anomaly correlation, for every level plane of every field, in one call.  Not a
+ * reference function: the reference's notebooks copy each prediction to the host and score it in numpy.
+ *
+ * One AbScoreField per variable (and batch member): `levels` planes of h x w float32 values in each of pred, truth and
+ * clim (clim may be NULL), row pitch ld_*, `*_level_stride` elements between planes.  Planes are numbered field by
+ * field, level by level.  For plane p, with w_r = row_weights[r] (double [h] of the largest h, DEVICE memory) and the
+ * point valid when pred, truth and (if given) clim are all not NaN, sums[p][0..7] =
+ *   W = sum w_r,  sum w_r d,  sum w_r d^2,  sum w_r |d|,  sum w_r af ao,  sum w_r af^2,  sum w_r ao^2,  count,
+ * over the valid points, d = double(pred) - double(truth), af = double(pred) - double(clim),
+ * ao = double(truth) - double(clim); the last three are 0 without clim.  +-inf is not skipped.  Every element is
+ * read once with float64 arithmetic; rows are split into a fixed (plane, row-chunk) partition whose partial sums go to
+ * `workspace` and are added in a fixed order by a second launch, so repeated calls give bit-identical sums (no
+ * atomics).  `fields` is a HOST array copied into the launch; `field_bytes` must be sizeof(AbScoreField);
+ * 1 <= n_fields <= AB_SCORE_MAX_FIELDS; h, w, levels >= 1, ld_* >= w; 16-byte loads where every pointer, pitch and
+ * level stride of a field allow, scalar loads otherwise.  `sums` is double [total planes][8], DEVICE memory.
+ * ---------------------------------------------------------------------------------------------- */
+#define AB_SCORE_MAX_FIELDS 64
+#define AB_SCORE_SUMS 8
+
+typedef struct AbScoreField {
+  const float* pred;  /* f32 [levels][h, ld_pred] */
+  const float* truth; /* f32 [levels][h, ld_truth] */
+  const float* clim;  /* f32 [levels][h, ld_clim] or NULL */
+  int64_t pred_level_stride, truth_level_stride, clim_level_stride; /* elements between consecutive levels */
+  int32_t h, w;
+  int32_t ld_pred, ld_truth, ld_clim;
+  int32_t levels;
+} AbScoreField;
+
+/* Workspace `ab_score_fields` needs for these fields (validates them like it does).  Host only. */
+int ab_score_workspace_bytes(const AbScoreField* fields, int32_t n_fields, size_t field_bytes, size_t* bytes);
+int ab_score_fields(const AbScoreField* fields, int32_t n_fields, size_t field_bytes, const double* row_weights,
+                    double* sums, void* workspace, size_t workspace_bytes, void* stream);
+
 /* sizeof() of the descriptor structs as this library was compiled (binding authors: compare with your mirror).
  * which: 0 AbGemm, 1 AbWindowAttention, 2 AbLnModResidual, 3 AbFieldIn, 4 AbFieldOut, 5 AbHaloPush, 6 AbSwinBlock,
  * 7 AbGemmLn, 8 AbPatchMergeLn, 9 AbPatchSplitLn, 10 AbOp; -1 for an unknown index.  Host only. */
