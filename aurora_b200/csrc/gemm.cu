@@ -11,15 +11,16 @@
 //
 // Pipelines: full / empty mbarriers per stage (TMA <-> wgmma) and the static persistent tile schedule
 // (tile = blockIdx.x + i * gridDim.x, N-blocks fastest so that the CTAs running concurrently share the same A rows in
-// L2 while W stays L2-resident), loaded by the producer in order.  Two ways to share it (see the kernel):
+// L2 while W stays L2-resident), loaded by the producer in order.  Three ways to share it (see the kernel):
 //   cooperative : both math warpgroups work on every 128 x BN tile, 64 rows each (BN = 64 / 128 / 256)
 //   ping-pong   : warpgroup w takes the positions i = w, w + 2, ... and all 128 rows of each 128 x 128 tile (two
 //                 m64n128k16 per k16 sharing the W descriptor); it starts a main loop only once the other has issued
 //                 the last k-block of its previous tile (two "order" mbarriers), so that one warpgroup's epilogue runs
 //                 while the other's wgmmas keep the tensor pipe busy
-// ab_gemm_bf16 takes ping-pong where the epilogue is a large part of a tile's time (K <= 1024, N > 128) and the
-// cooperative tile elsewhere, whose wgmmas read fewer shared-memory bytes per FLOP.  One wgmma group stays in flight
-// while the next stage is waited for.
+//   staggered   : the cooperative 128 x 256 tile, with warpgroup 1 kept 1-2 k-blocks behind warpgroup 0 (two rings of
+//                 "issued" mbarriers), so that each warpgroup's epilogue runs under the other's wgmmas for that long
+// ab_gemm_bf16 runs every shape cooperative (see the reason there); AB_GEMM_SCHEDULE forces one of the three for tools
+// and tests.  One wgmma group stays in flight while the next stage is waited for.
 //
 // Phase trace: built with -DAB_GEMM_TRACE (tools/gemm_trace.py does that into build/trace/), the kernel sums
 // clock64() cycles per warp role and phase in registers and writes them once per CTA into a device buffer set with
@@ -43,21 +44,32 @@ constexpr int kNumThreads = 128 + kMathWarps * 32;
 constexpr int kBoxRows = 16;   // rows of one epilogue box = rows of one m64 accumulator that one warp holds
 constexpr int kBoxBytes = kBoxRows * 128;
 
-template <int BN, bool kPingPong>
+enum Schedule { kCooperative, kPingPong, kStaggered };
+
+// Staggered schedule: warpgroup 1 issues ring position p only once warpgroup 0 has issued p + kLagMin (or the last
+// k-block of p's tile), and warpgroup 0 issues p only once warpgroup 1 has issued p - kLagMax.  kLagMax = 2 of the
+// 4 stages leaves the producer one stage of prefetch ahead of warpgroup 0.
+constexpr int kLagMin = 1;
+constexpr int kLagMax = 2;
+
+template <int BN, int kSched>
 struct GemmCfg {
   static constexpr int kStageBytesA = kBlockM * kBlockK * 2;
   static constexpr int kStageBytesB = BN * kBlockK * 2;
   static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
   static constexpr int kStages = BN >= 256 ? 4 : (BN >= 128 ? 6 : 8);
-  static constexpr int kBarrierBytes = 256;
+  // full + empty per stage, 2 order (ping-pong); staggered adds one "issued" ring per warpgroup
+  static constexpr int kBarriers = 2 * kStages + 2 + (kSched == kStaggered ? 2 * kStages : 0);
+  static constexpr int kBarrierBytes = kBarriers * 8;
   static constexpr int kStagingBytes = kMathWarps * 2 * kBoxBytes;  // two 16-row x 128-byte store boxes per math warp
-  // the tile's BN bias values: one copy per warpgroup for ping-pong (each has its own tile), one for cooperative
-  static constexpr int kBiasGroups = kPingPong ? 2 : 1;
+  // the tile's BN bias values: one copy per warpgroup where the two warpgroups reach their epilogues at different
+  // times (ping-pong: different tiles; staggered: the same tile, k-blocks apart), one for cooperative
+  static constexpr int kBiasGroups = kSched == kCooperative ? 1 : 2;
   static constexpr int kBiasThreads = kMathWarps * 32 / kBiasGroups;  // the math threads that share a copy
   static constexpr int kBiasBytes = kBiasGroups * BN * 4;
-  static constexpr int kSmemBytes =
-      kStages * kStageBytes + kStagingBytes + kBiasBytes + kBarrierBytes + 1024;  // +1024: alignment
-  static_assert((2 * kStages + 2) * 8 <= kBarrierBytes, "barrier area");
+  // no alignment slack: smem_raw is declared 1024-byte aligned (staggered BN = 256 needs all but 880 bytes of 227 KB)
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBiasBytes + kBarrierBytes;
+  static_assert(kSched != kStaggered || (kStages > kLagMax + 1 && kLagMin < kLagMax), "lag bounds (see the kernel)");
   static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 };
 
@@ -66,7 +78,7 @@ enum TraceCta { kTrTimerStart, kTrTimerEnd, kTrClockStart, kTrClockEnd, kTrEmpty
 enum TraceSlot {
   kTrFullFirst,  // full_bar wait of a tile's first k-block (producer: empty_bar waits)
   kTrFullRest,   // full_bar waits of its other k-blocks
-  kTrOrder,      // order_bar wait (ping-pong)
+  kTrOrder,      // order_bar wait (ping-pong), lead_bar / follow_bar waits (staggered)
   kTrWait1,      // wgmma_wait<1> in the main loop
   kTrWait0,      // wgmma_wait<0> after it
   kTrEpi,        // the whole epilogue
@@ -324,20 +336,46 @@ __device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMa
   }
 }
 
-// kPingPong = false, "cooperative": both math warpgroups work on every tile of the CTA, warpgroup w on rows
-//   [64 w, 64 w + 64) (one m64nBNk16 accumulator each, BN up to 256).
-// kPingPong = true: warpgroup w takes the tiles at positions w, w + 2, ... of the CTA's sequence and all 128 rows of
-//   each (two m64nBNk16 accumulators, BN = 128); it starts a main loop only once the other warpgroup has issued the
-//   last k-block of the tile before, so that one warpgroup's epilogue runs under the other's wgmmas.
-template <int BN, bool kPingPong, bool kHalfIn>
+// kCooperative: both math warpgroups work on every tile of the CTA, warpgroup w on rows [64 w, 64 w + 64) (one
+//   m64nBNk16 accumulator each, BN up to 256).
+// kPingPong: warpgroup w takes the tiles at positions w, w + 2, ... of the CTA's sequence and all 128 rows of each (two
+//   m64nBNk16 accumulators, BN = 128); it starts a main loop only once the other warpgroup has issued the last k-block
+//   of the tile before, so that one warpgroup's epilogue runs under the other's wgmmas.
+// kStaggered: the cooperative tile and stage ring (every stage is freed by all 8 math warps), with warpgroup 0 ("the
+//   leader") kept between kLagMin and kLagMax k-blocks ahead of warpgroup 1 ("the follower").  Ring position p is
+//   the CTA's p-th k-block, the same sequence for both warpgroups; after issuing p each warpgroup arrives on its own
+//   "issued" ring (lead_bar / follow_bar [p mod S], one arrival per warp, phase p / S).  Before issuing p:
+//     leader   waits until the follower has issued p - kLagMax (the upper bound: the follower's releases keep the
+//              producer kLagMax - 1 stages ahead of the leader, so the leader does not wait on TMA latency);
+//     follower waits until the leader has issued min(p + kLagMin, last k-block of p's tile) (the lower bound, clamped
+//              to the tile: the follower never waits for the leader's epilogue).
+//   So the follower's last k-blocks of a tile run under the leader's epilogue, and the leader's first kLagMax
+//   k-blocks of the next tile under the follower's epilogue.  Each warpgroup stages its own bias copy, with its own
+//   named barrier: the two never synchronise except through the rings.
+//   No deadlock (S = kStages, kLagMin < kLagMax < S - 1; a warpgroup frees p right after issuing p + 1, or after its
+//   wgmma_wait<0> when p ends its tile, with no wait in between).  Let the leader wait at a, the follower at b:
+//     - leader on the follower (b <= a - kLagMax): the follower needs the leader at b + kLagMin < a, issued, and
+//       stage b, which needs b - S freed by both: the leader issued up to a - 1 > b - S + 1, the follower up to b - 1.
+//     - leader on stage a: needs a - S freed by the follower, so b <= a - S + 1; the follower needs the leader at
+//       <= b + kLagMin < a (issued) and stage b (b - S freed by both, as above).
+//     - follower on the leader (a <= min(b + kLagMin, end)): the leader needs the follower at a - kLagMax < b
+//       (issued) and stage a: a - S <= b + kLagMin - S < b - 1 is freed by both.
+//   Each case names a wait that the blocked warpgroup's partner or the producer can satisfy without waiting on the
+//   first, so the three always progress.  Both take every tile of the CTA, so the sequence is the same whatever the
+//   tile count, K (one k-block included: the lower bound then points inside the same tile) or M tail (rows past M are
+//   zero-filled by TMA and computed as usual).  Parity: when the follower waits on lead_bar for q, the leader has
+//   issued q - S (the follower's previous wait) and cannot issue q + S (stage q + S needs the follower to free q);
+//   symmetrically for follow_bar, so the wait never sees a phase too early or too late.
+template <int BN, int kSched, bool kHalfIn>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_out, const GemmArgs g) {
-  using Cfg = GemmCfg<BN, kPingPong>;
-  constexpr int kRB = kPingPong ? 2 : 1;  // 64-row accumulator blocks per warpgroup
-  extern __shared__ uint8_t smem_raw[];
-  // 128B-swizzled tiles need 1024-byte alignment.
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  using Cfg = GemmCfg<BN, kSched>;
+  constexpr bool kPP = kSched == kPingPong;
+  constexpr bool kStag = kSched == kStaggered;
+  constexpr int kRB = kPP ? 2 : 1;  // 64-row accumulator blocks per warpgroup
+  extern __shared__ __align__(1024) uint8_t smem_raw[];  // 128B-swizzled tiles need 1024-byte alignment
+  uint8_t* smem = smem_raw;
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kStageBytesA;
   uint8_t* smem_stage_out = smem + Cfg::kStages * Cfg::kStageBytes;  // 1024-byte aligned (stages are)
@@ -345,6 +383,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes + Cfg::kBiasBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
   uint64_t* order_bar = empty_bar + Cfg::kStages;  // ping-pong, [w]: math warpgroup w may start its next main loop
+  uint64_t* lead_bar = order_bar + 2;               // staggered, [p mod S]: the leader has issued ring position p
+  uint64_t* follow_bar = lead_bar + Cfg::kStages;   // staggered: the follower has issued p
 
   const int warp = threadIdx.x >> 5;  // warp-uniform
   const int lane = threadIdx.x & 31;
@@ -363,7 +403,11 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     if (g.tma_out) prefetch_tmap(&tmap_out);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kPingPong ? 4 : kMathWarps);  // the warps that consume the stage
+      mbar_init(&empty_bar[s], kPP ? 4 : kMathWarps);  // the warps that consume the stage
+      if (kStag) {
+        mbar_init(&lead_bar[s], 4);
+        mbar_init(&follow_bar[s], 4);
+      }
     }
     mbar_init(&order_bar[0], 4);
     mbar_init(&order_bar[1], 4);
@@ -406,17 +450,21 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     reg_alloc<232>();
     const int wg = (warp >> 2) - 1;
     // first of this warp's 16 rows inside the tile (inside each 64-row block for ping-pong)
-    const int warp_row = (kPingPong ? 0 : wg * 64) + (warp & 3) * kBoxRows;
+    const int warp_row = (kPP ? 0 : wg * 64) + (warp & 3) * kBoxRows;
     uint8_t* const staging = smem_stage_out + (warp - 4) * (2 * kBoxBytes);
-    // the bias copy of this warp's group (ping-pong: its warpgroup; cooperative: both) and the group's named barrier
-    const int bias_group = kPingPong ? wg : 0;
+    // the bias copy of this warp's group (ping-pong / staggered: its warpgroup; cooperative: both) and the group's
+    // named barrier
+    const int bias_group = kSched == kCooperative ? 0 : wg;
     float* const bias_s = smem_bias + bias_group * BN;
     const int bias_tid = threadIdx.x - 128 - bias_group * Cfg::kBiasThreads;
+    // staggered: the ring this warpgroup signals after issuing a k-block, and the one it waits on
+    uint64_t* const issued_bar = wg == 0 ? lead_bar : follow_bar;
+    uint64_t* const partner_bar = wg == 0 ? follow_bar : lead_bar;
     float acc[kRB][BN / 2];
     uint32_t nst = 0;  // TMA stores this warp has issued: picks the staging buffer
-    constexpr int kStep = kPingPong ? 2 : 1;
+    constexpr int kStep = kPP ? 2 : 1;
     uint32_t j = 0;  // tiles this warpgroup has taken
-    for (int i = kPingPong ? wg : 0;; i += kStep, ++j) {
+    for (int i = kPP ? wg : 0;; i += kStep, ++j) {
       const int tile = blockIdx.x + i * gridDim.x;
       if (tile >= num_tiles) break;
       const int m0 = (tile / num_n) * kBlockM;
@@ -426,20 +474,27 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         stage_bias<BN, Cfg::kBiasThreads>(g, bias_s, n0, bias_tid);
       }
       // ping-pong: tile i - 1 (the other warpgroup's) has issued all its wgmmas
-      if (kPingPong && i > 0) {
+      if (kPP && i > 0) {
         const long long t0 = tr.now();
         mbar_wait(&order_bar[wg], (wg == 0 ? j - 1 : j) & 1u);
         tr.add(kTrOrder, t0);
       }
       uint32_t it = static_cast<uint32_t>(i) * num_kb;  // the ring position of this tile's first k-block
+      const uint32_t it_last = it + num_kb - 1;
       int prev_s = -1;
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const uint32_t s = it % Cfg::kStages;
+        if (kStag && (wg == 1 || it >= kLagMax)) {  // the lag bounds (see the kernel comment)
+          const uint32_t q = wg == 0 ? it - kLagMax : min(it + kLagMin, it_last);
+          const long long t0 = tr.now();
+          mbar_wait(&partner_bar[q % Cfg::kStages], (q / Cfg::kStages) & 1u);
+          tr.add(kTrOrder, t0);
+        }
         const long long t0 = tr.now();
         mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1u);
         if (kb == 0) tr.add(kTrFullFirst, t0);
         else tr.add(kTrFullRest, t0);
-        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + (kPingPong ? 0 : wg * (64 * 128));
+        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + (kPP ? 0 : wg * (64 * 128));
         const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
 #pragma unroll
         for (int rb = 0; rb < kRB; ++rb) wgmma_fence_regs(acc[rb]);
@@ -453,7 +508,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
                                   (kb | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
-        if (kPingPong && kb == num_kb - 1 && lane == 0) mbar_arrive(&order_bar[wg ^ 1]);  // hand the tensor pipe over
+        if (kPP && kb == num_kb - 1 && lane == 0) mbar_arrive(&order_bar[wg ^ 1]);  // hand the tensor pipe over
+        if (kStag && lane == 0) mbar_arrive(&issued_bar[s]);
         if (prev_s >= 0) {
           const long long t1 = tr.now();
           wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand its shared memory back to the producer
@@ -504,9 +560,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 static unsigned long long* g_trace_buf = nullptr;
 #endif
 
-template <int BN, bool kPingPong, bool kHalfIn>
+template <int BN, int kSched, bool kHalfIn>
 static int launch_gemm(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, kPingPong>;
+  using Cfg = GemmCfg<BN, kSched>;
   CUtensorMap ta, tw;
   int rc = make_tmap_16bit_2d(&ta, p->a, p->m, p->k, p->lda, kBlockM, kBlockK, kHalfIn);
   if (rc != AB_OK) return rc;
@@ -519,7 +575,7 @@ static int launch_gemm(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, kPingPong, kHalfIn>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, kSched, kHalfIn>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("ab_gemm_bf16: cudaFuncSetAttribute(smem=%d) failed: %s", Cfg::kSmemBytes, cudaGetErrorString(e));
@@ -533,10 +589,39 @@ static int launch_gemm(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
   AB_CHECK_ARG(g_trace_buf != nullptr, "ab_gemm_bf16: traced build without a trace buffer (ab_gemm_trace)");
   args.trace = g_trace_buf;
 #endif
-  gemm_bf16_tn_kernel<BN, kPingPong, kHalfIn><<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
+  gemm_bf16_tn_kernel<BN, kSched, kHalfIn><<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
   AB_COUNT_LAUNCH(1);
   AB_CHECK_LAUNCH("ab_gemm_bf16");
   return AB_OK;
+}
+
+// The tile shape of each schedule: 128 x 128 per warpgroup for ping-pong, 128 x 256 per CTA for cooperative and
+// staggered while N > 128, 128 x 128 / 128 x 64 cooperative for the narrower decoder heads.
+template <bool kHalfIn>
+static int launch_for(const AbGemm* p, GemmArgs& args, cudaStream_t stream, int sched) {
+  if (p->n > 128) {
+    if (sched == kPingPong) return launch_gemm<128, kPingPong, kHalfIn>(p, args, stream);
+    if (sched == kStaggered) return launch_gemm<256, kStaggered, kHalfIn>(p, args, stream);
+    return launch_gemm<256, kCooperative, kHalfIn>(p, args, stream);
+  }
+  if (p->n > 64) return launch_gemm<128, kCooperative, kHalfIn>(p, args, stream);
+  return launch_gemm<64, kCooperative, kHalfIn>(p, args, stream);
+}
+
+// AB_GEMM_SCHEDULE=pingpong|cooperative|staggered, read once: every GEMM with N > 128 takes that schedule instead of
+// the rule in ab_gemm_bf16, so that tools and tests can compare the schedules on the same shapes.  The model never
+// sets it.  -1: unset.
+constexpr int kBadSchedule = -2;
+static int forced_schedule() {
+  static const int forced = [] {
+    const char* e = getenv("AB_GEMM_SCHEDULE");
+    if (e == nullptr || *e == 0) return -1;
+    if (strcmp(e, "pingpong") == 0) return static_cast<int>(kPingPong);
+    if (strcmp(e, "cooperative") == 0) return static_cast<int>(kCooperative);
+    if (strcmp(e, "staggered") == 0) return static_cast<int>(kStaggered);
+    return kBadSchedule;
+  }();
+  return forced;
 }
 
 #ifdef AB_GEMM_TRACE
@@ -645,19 +730,17 @@ extern "C" int ab_gemm_bf16(const AbGemm* p, void* stream) {
     pr.expected = groups * ((p->n - pr.col_from + 63) / 64);
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  // Ping-pong for K <= 1024 and N > 128: there the epilogue is a large part of a tile's time and runs hidden under the
-  // other warpgroup's main loop.  From K = 2048 on the cooperative 128 x 256 tile is as fast or faster: its wgmmas read
-  // fewer shared-memory bytes per FLOP (B once for 128 rows, 48 KB of operands per 128 x 256 x 64 step against 32 KB
-  // per 128 x 128 x 64), and the main loop dominates.  The decoder heads (N = 80 and 64) stay cooperative as well.
-  const bool ping_pong = p->n > 128 && p->k <= 1024;
-  if (p->in_dtype == AB_DT_F16) {
-    if (ping_pong) return launch_gemm<128, true, true>(p, a, s);
-    if (p->n > 128) return launch_gemm<256, false, true>(p, a, s);
-    if (p->n > 64) return launch_gemm<128, false, true>(p, a, s);
-    return launch_gemm<64, false, true>(p, a, s);
-  }
-  if (ping_pong) return launch_gemm<128, true, false>(p, a, s);
-  if (p->n > 128) return launch_gemm<256, false, false>(p, a, s);
-  if (p->n > 64) return launch_gemm<128, false, false>(p, a, s);
-  return launch_gemm<64, false, false>(p, a, s);
+  // Every shape takes the cooperative tile (128 x 256 for N > 128).  Since the epilogue no longer waits on global loads
+  // or on its stores (3.3 us per 128 x 256 tile, 4.9-5.3 us with GELU), the cooperative main loop, whose wgmmas read
+  // fewer shared-memory bytes per FLOP (48 KB of operands per 128 x 256 x 64 step against 32 KB per 128 x 128 x 64),
+  // costs less than the ping-pong tile's hidden epilogue saves: with every shape cooperative the 0.25-degree step ran
+  // 3 % faster than with ping-pong at K <= 1024, and ping-pong at K <= 1024 for N <= 1024 only was no better (DESIGN
+  // §6).  Staggered loses to both: its lag waits cost more than the epilogue time it hides.  Both stay for
+  // AB_GEMM_SCHEDULE.
+  int sched = kCooperative;
+  const int forced = forced_schedule();
+  AB_CHECK_ARG(forced != kBadSchedule, "ab_gemm_bf16: AB_GEMM_SCHEDULE must be pingpong, cooperative or staggered");
+  if (forced >= 0 && p->n > 128) sched = forced;
+  if (p->in_dtype == AB_DT_F16) return launch_for<true>(p, a, s, sched);
+  return launch_for<false>(p, a, s, sched);
 }

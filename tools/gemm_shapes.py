@@ -11,6 +11,8 @@
    main-loop rate; `fixed_share` is t0 over the time at the shape's own K.
 4. The card: name, power limit and max SM clock, read in the same run.
 
+AB_GEMM_SCHEDULE=pingpong|cooperative|staggered in the environment times every N > 128 shape on that schedule.
+
 Writes nothing; needs a GPU.
 """
 

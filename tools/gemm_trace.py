@@ -13,13 +13,15 @@
      producer         empty_bar waits of the TMA producer
      full_first       full_bar wait of a tile's first k-block    |
      full_rest        full_bar waits of its other k-blocks        |
-     order            order_bar wait (ping-pong)                  |  per math warp, over the tiles
+     order            order_bar wait (ping-pong), lag waits       |  per math warp, over the tiles
+                      (staggered)                                 |
      wait1 / wait0    wgmma_wait<1> / <0>                         |  that warp's warpgroup took
      epilogue         the whole epilogue, of which                |
        store_wait     waits for a store buffer                    |
        bias_wait      waits for the bias values                   |
        math_store     the rest: bias, GELU, packing, stores       |
    plus the card line (name, power limit, max SM clock) from the same run.
+   AB_GEMM_SCHEDULE=pingpong|cooperative|staggered in the environment traces that schedule (N > 128 shapes).
 
 Writes build/trace/ only; needs a GPU to run.
 """
