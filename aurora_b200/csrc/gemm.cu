@@ -11,23 +11,17 @@
 //
 // Pipelines: full / empty mbarriers per stage (TMA <-> wgmma) and the static persistent tile schedule
 // (tile = blockIdx.x + i * gridDim.x, N-blocks fastest so that the CTAs running concurrently share the same A rows in
-// L2 while W stays L2-resident), loaded by the producer in order.  Three ways to share it (see the kernel):
-//   cooperative : both math warpgroups work on every 128 x BN tile, 64 rows each (BN = 64 / 128 / 256)
-//   ping-pong   : warpgroup w takes the positions i = w, w + 2, ... and all 128 rows of each 128 x 128 tile (two
-//                 m64n128k16 per k16 sharing the W descriptor); it starts a main loop only once the other has issued
-//                 the last k-block of its previous tile (two "order" mbarriers), so that one warpgroup's epilogue runs
-//                 while the other's wgmmas keep the tensor pipe busy
-//   staggered   : the cooperative 128 x 256 tile, with warpgroup 1 kept 1-2 k-blocks behind warpgroup 0 (two rings of
-//                 "issued" mbarriers), so that each warpgroup's epilogue runs under the other's wgmmas for that long
-// ab_gemm_bf16 runs every shape cooperative (see the reason there); AB_GEMM_SCHEDULE forces one of the three for tools
-// and tests.  One wgmma group stays in flight while the next stage is waited for.
+// L2 while W stays L2-resident), loaded by the producer in order.  Both math warpgroups work on every 128 x BN tile,
+// warpgroup w on rows [64 w, 64 w + 64) (BN = 256 for N > 128, 128 / 64 for the decoder heads), and every stage is
+// freed by all 8 math warps.  One wgmma group stays in flight while the next stage is waited for.  Two other schedules,
+// ping-pong (alternate 128 x 128 tiles per warpgroup) and staggered (warpgroup 1 held 1-2 k-blocks behind warpgroup 0),
+// hid part of the epilogue under the other warpgroup's wgmmas and were slower on the whole step (DESIGN §6).
 //
 // Phase trace: built with -DAB_GEMM_TRACE (tools/gemm_trace.py does that into build/trace/), the kernel sums
 // clock64() cycles per warp role and phase in registers and writes them once per CTA into a device buffer set with
 // ab_gemm_trace(); without the switch the trace code compiles to nothing.
 //
 // Replaces: every nn.Linear on Aurora's forward path (see include/aurora_b200.h).
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.h"
@@ -39,37 +33,24 @@ namespace ab {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 bytes = one swizzle row
 constexpr int kWgmmaK = 16;
-constexpr int kMathWarps = 8;  // two warpgroups, one tile each
-constexpr int kNumThreads = 128 + kMathWarps * 32;
+constexpr int kMathWarps = 8;  // two warpgroups, 64 rows of the tile each
+constexpr int kMathThreads = kMathWarps * 32;
+constexpr int kNumThreads = 128 + kMathThreads;
 constexpr int kBoxRows = 16;   // rows of one epilogue box = rows of one m64 accumulator that one warp holds
 constexpr int kBoxBytes = kBoxRows * 128;
 
-enum Schedule { kCooperative, kPingPong, kStaggered };
-
-// Staggered schedule: warpgroup 1 issues ring position p only once warpgroup 0 has issued p + kLagMin (or the last
-// k-block of p's tile), and warpgroup 0 issues p only once warpgroup 1 has issued p - kLagMax.  kLagMax = 2 of the
-// 4 stages leaves the producer one stage of prefetch ahead of warpgroup 0.
-constexpr int kLagMin = 1;
-constexpr int kLagMax = 2;
-
-template <int BN, int kSched>
+template <int BN>
 struct GemmCfg {
   static constexpr int kStageBytesA = kBlockM * kBlockK * 2;
   static constexpr int kStageBytesB = BN * kBlockK * 2;
   static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
   static constexpr int kStages = BN >= 256 ? 4 : (BN >= 128 ? 6 : 8);
-  // full + empty per stage, 2 order (ping-pong); staggered adds one "issued" ring per warpgroup
-  static constexpr int kBarriers = 2 * kStages + 2 + (kSched == kStaggered ? 2 * kStages : 0);
+  static constexpr int kBarriers = 2 * kStages;  // full + empty per stage
   static constexpr int kBarrierBytes = kBarriers * 8;
   static constexpr int kStagingBytes = kMathWarps * 2 * kBoxBytes;  // two 16-row x 128-byte store boxes per math warp
-  // the tile's BN bias values: one copy per warpgroup where the two warpgroups reach their epilogues at different
-  // times (ping-pong: different tiles; staggered: the same tile, k-blocks apart), one for cooperative
-  static constexpr int kBiasGroups = kSched == kCooperative ? 1 : 2;
-  static constexpr int kBiasThreads = kMathWarps * 32 / kBiasGroups;  // the math threads that share a copy
-  static constexpr int kBiasBytes = kBiasGroups * BN * 4;
-  // no alignment slack: smem_raw is declared 1024-byte aligned (staggered BN = 256 needs all but 880 bytes of 227 KB)
+  static constexpr int kBiasBytes = BN * 4;                          // the tile's BN bias values
+  // no alignment slack: smem_raw is declared 1024-byte aligned (BN = 256 needs all but 1984 bytes of 227 KB)
   static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kBiasBytes + kBarrierBytes;
-  static_assert(kSched != kStaggered || (kStages > kLagMax + 1 && kLagMin < kLagMax), "lag bounds (see the kernel)");
   static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 };
 
@@ -78,7 +59,6 @@ enum TraceCta { kTrTimerStart, kTrTimerEnd, kTrClockStart, kTrClockEnd, kTrEmpty
 enum TraceSlot {
   kTrFullFirst,  // full_bar wait of a tile's first k-block (producer: empty_bar waits)
   kTrFullRest,   // full_bar waits of its other k-blocks
-  kTrOrder,      // order_bar wait (ping-pong), lead_bar / follow_bar waits (staggered)
   kTrWait1,      // wgmma_wait<1> in the main loop
   kTrWait0,      // wgmma_wait<0> after it
   kTrEpi,        // the whole epilogue
@@ -224,12 +204,12 @@ __device__ __forceinline__ void epilogue_direct(const GemmArgs& g, float (&acc)[
   }
 }
 
-// Copy of the tile's bias values n0 .. n0 + BN into the group's shared-memory slice, asynchronously (cp.async, 16 bytes
-// per thread, waited for at the epilogue); columns past N read 0.  Issued at the start of a tile so that the epilogue
-// has no global load: a bias __ldg there waits on L2 once per box.  kThreads: the math threads that share the slice.
-template <int BN, int kThreads>
+// Copy of the tile's bias values n0 .. n0 + BN into shared memory, asynchronously (cp.async, 16 bytes per thread, waited
+// for at the epilogue); columns past N read 0.  Issued at the start of a tile so that the epilogue has no global load:
+// a bias __ldg there waits on L2 once per box.  tid: the index of the math thread.
+template <int BN>
 __device__ __forceinline__ void stage_bias(const GemmArgs& g, float* bias_s, int n0, int tid) {
-  static_assert(BN / 4 <= kThreads, "one 16-byte copy per thread");
+  static_assert(BN / 4 <= kMathThreads, "one 16-byte copy per thread");
   if (tid < BN / 4) {
     const int col = n0 + 4 * tid;
     const int bytes = col >= g.n ? 0 : (g.n - col >= 4 ? 16 : 4 * (g.n - col));
@@ -240,20 +220,18 @@ __device__ __forceinline__ void stage_bias(const GemmArgs& g, float* bias_s, int
   asm volatile("cp.async.commit_group;" ::: "memory");
 }
 
-// Named barrier of the kThreads math threads that share a bias slice (id 0 is __syncthreads).
-template <int kThreads>
-__device__ __forceinline__ void group_sync(int id) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(kThreads) : "memory");
+// Named barrier 1 of the math threads, which share the bias copy (id 0 is __syncthreads).
+__device__ __forceinline__ void math_sync() {
+  asm volatile("bar.sync %0, %1;" ::"r"(1), "n"(kMathThreads) : "memory");
 }
 
 // 16-bit-only epilogue of one 16-row x 64-column box (rows row0 .. row0 + 15 of the output, columns colb ..): bias (from
-// the group's shared-memory copy) / activation on the registers, 16-bit pairs into one of this warp's two staging boxes
-// (16 rows x 128 bytes, 128B swizzle: chunk ^= row & 7, the layout a CU_TENSOR_MAP_SWIZZLE_128B store expects), then
-// one asynchronous TMA store: full 128-byte rows, M / N tails clipped by the tensor map.  The staging stores are
-// stmatrix, 4 per box where 32-bit stores would take 16: in ping-pong they queue for shared memory behind the other
-// warpgroup's wgmma operand reads, and fewer of them shorten the epilogue (4.8 against 5.0 µs per tile, stage-1 qkv).  The two buffers alternate per issued
-// store, so filling one only waits for the store issued two boxes ago.  Rows that a neighbouring GPU needs are copied
-// out of the staging box into its halo slot, 16 bytes per lane.
+// the shared-memory copy) / activation on the registers, 16-bit pairs into one of this warp's two staging boxes (16 rows
+// x 128 bytes, 128B swizzle: chunk ^= row & 7, the layout a CU_TENSOR_MAP_SWIZZLE_128B store expects), then one
+// asynchronous TMA store: full 128-byte rows, M / N tails clipped by the tensor map.  The staging stores are stmatrix,
+// 4 per box where 32-bit stores would take 16; fewer of them shorten the epilogue (4.8 against 5.0 µs per 128 x 128
+// tile, stage-1 qkv).  The two buffers alternate per issued store, so filling one only waits for the store issued two
+// boxes ago.  Rows that a neighbouring GPU needs are copied out of the staging box into its halo slot, 16 bytes per lane.
 template <int BN>
 __device__ __forceinline__ void epilogue_tma_box(const GemmArgs& g, const CUtensorMap* tmap_out, const float (&acc)[BN / 2],
                                                  const float* bias_s, int c, uint8_t* staging, uint32_t& nst,
@@ -321,59 +299,26 @@ __device__ __forceinline__ void epilogue_tma_box(const GemmArgs& g, const CUtens
   ++nst;
 }
 
-// 16-bit-only epilogue of a warpgroup's kRB x 64 rows: per 64-column box, each 64-row block in turn.
-template <int BN, int kRB>
-__device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmap_out, const float (&acc)[kRB][BN / 2],
-                                             const float* bias_s, uint8_t* staging, uint32_t& nst, int warp_row0,
-                                             int n0, int lane, Trace& tr) {
+// 16-bit-only epilogue of a warp's 16 rows of the tile: one box per 64-column block.
+template <int BN>
+__device__ __forceinline__ void epilogue_tma(const GemmArgs& g, const CUtensorMap* tmap_out, const float (&acc)[BN / 2],
+                                             const float* bias_s, uint8_t* staging, uint32_t& nst, int row0, int n0,
+                                             int lane, Trace& tr) {
 #pragma unroll
   for (int c = 0; c < BN / 64; ++c) {
     const int colb = n0 + 64 * c;
     if (colb >= g.n) continue;  // warp-uniform
-#pragma unroll
-    for (int rb = 0; rb < kRB; ++rb)
-      epilogue_tma_box<BN>(g, tmap_out, acc[rb], bias_s, c, staging, nst, warp_row0 + 64 * rb, colb, lane, tr);
+    epilogue_tma_box<BN>(g, tmap_out, acc, bias_s, c, staging, nst, row0, colb, lane, tr);
   }
 }
 
-// kCooperative: both math warpgroups work on every tile of the CTA, warpgroup w on rows [64 w, 64 w + 64) (one
-//   m64nBNk16 accumulator each, BN up to 256).
-// kPingPong: warpgroup w takes the tiles at positions w, w + 2, ... of the CTA's sequence and all 128 rows of each (two
-//   m64nBNk16 accumulators, BN = 128); it starts a main loop only once the other warpgroup has issued the last k-block
-//   of the tile before, so that one warpgroup's epilogue runs under the other's wgmmas.
-// kStaggered: the cooperative tile and stage ring (every stage is freed by all 8 math warps), with warpgroup 0 ("the
-//   leader") kept between kLagMin and kLagMax k-blocks ahead of warpgroup 1 ("the follower").  Ring position p is
-//   the CTA's p-th k-block, the same sequence for both warpgroups; after issuing p each warpgroup arrives on its own
-//   "issued" ring (lead_bar / follow_bar [p mod S], one arrival per warp, phase p / S).  Before issuing p:
-//     leader   waits until the follower has issued p - kLagMax (the upper bound: the follower's releases keep the
-//              producer kLagMax - 1 stages ahead of the leader, so the leader does not wait on TMA latency);
-//     follower waits until the leader has issued min(p + kLagMin, last k-block of p's tile) (the lower bound, clamped
-//              to the tile: the follower never waits for the leader's epilogue).
-//   So the follower's last k-blocks of a tile run under the leader's epilogue, and the leader's first kLagMax
-//   k-blocks of the next tile under the follower's epilogue.  Each warpgroup stages its own bias copy, with its own
-//   named barrier: the two never synchronise except through the rings.
-//   No deadlock (S = kStages, kLagMin < kLagMax < S - 1; a warpgroup frees p right after issuing p + 1, or after its
-//   wgmma_wait<0> when p ends its tile, with no wait in between).  Let the leader wait at a, the follower at b:
-//     - leader on the follower (b <= a - kLagMax): the follower needs the leader at b + kLagMin < a, issued, and
-//       stage b, which needs b - S freed by both: the leader issued up to a - 1 > b - S + 1, the follower up to b - 1.
-//     - leader on stage a: needs a - S freed by the follower, so b <= a - S + 1; the follower needs the leader at
-//       <= b + kLagMin < a (issued) and stage b (b - S freed by both, as above).
-//     - follower on the leader (a <= min(b + kLagMin, end)): the leader needs the follower at a - kLagMax < b
-//       (issued) and stage a: a - S <= b + kLagMin - S < b - 1 is freed by both.
-//   Each case names a wait that the blocked warpgroup's partner or the producer can satisfy without waiting on the
-//   first, so the three always progress.  Both take every tile of the CTA, so the sequence is the same whatever the
-//   tile count, K (one k-block included: the lower bound then points inside the same tile) or M tail (rows past M are
-//   zero-filled by TMA and computed as usual).  Parity: when the follower waits on lead_bar for q, the leader has
-//   issued q - S (the follower's previous wait) and cannot issue q + S (stage q + S needs the follower to free q);
-//   symmetrically for follow_bar, so the wait never sees a phase too early or too late.
-template <int BN, int kSched, bool kHalfIn>
+// Both math warpgroups work on every tile of the CTA, warpgroup w on rows [64 w, 64 w + 64) (one m64nBNk16 accumulator
+// each, BN up to 256).
+template <int BN, bool kHalfIn>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ CUtensorMap tmap_out, const GemmArgs g) {
-  using Cfg = GemmCfg<BN, kSched>;
-  constexpr bool kPP = kSched == kPingPong;
-  constexpr bool kStag = kSched == kStaggered;
-  constexpr int kRB = kPP ? 2 : 1;  // 64-row accumulator blocks per warpgroup
+  using Cfg = GemmCfg<BN>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];  // 128B-swizzled tiles need 1024-byte alignment
   uint8_t* smem = smem_raw;
   uint8_t* smem_a = smem;
@@ -382,9 +327,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   float* smem_bias = reinterpret_cast<float*>(smem_stage_out + Cfg::kStagingBytes);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stage_out + Cfg::kStagingBytes + Cfg::kBiasBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* order_bar = empty_bar + Cfg::kStages;  // ping-pong, [w]: math warpgroup w may start its next main loop
-  uint64_t* lead_bar = order_bar + 2;               // staggered, [p mod S]: the leader has issued ring position p
-  uint64_t* follow_bar = lead_bar + Cfg::kStages;   // staggered: the follower has issued p
 
   const int warp = threadIdx.x >> 5;  // warp-uniform
   const int lane = threadIdx.x & 31;
@@ -403,14 +345,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     if (g.tma_out) prefetch_tmap(&tmap_out);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kPP ? 4 : kMathWarps);  // the warps that consume the stage
-      if (kStag) {
-        mbar_init(&lead_bar[s], 4);
-        mbar_init(&follow_bar[s], 4);
-      }
+      mbar_init(&empty_bar[s], kMathWarps);  // the warps that consume the stage
     }
-    mbar_init(&order_bar[0], 4);
-    mbar_init(&order_bar[1], 4);
     fence_mbar_init();
   }
   __syncthreads();
@@ -449,67 +385,37 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     // ===== math warpgroups =====
     reg_alloc<232>();
     const int wg = (warp >> 2) - 1;
-    // first of this warp's 16 rows inside the tile (inside each 64-row block for ping-pong)
-    const int warp_row = (kPP ? 0 : wg * 64) + (warp & 3) * kBoxRows;
+    const int warp_row = wg * 64 + (warp & 3) * kBoxRows;  // first of this warp's 16 rows inside the tile
     uint8_t* const staging = smem_stage_out + (warp - 4) * (2 * kBoxBytes);
-    // the bias copy of this warp's group (ping-pong / staggered: its warpgroup; cooperative: both) and the group's
-    // named barrier
-    const int bias_group = kSched == kCooperative ? 0 : wg;
-    float* const bias_s = smem_bias + bias_group * BN;
-    const int bias_tid = threadIdx.x - 128 - bias_group * Cfg::kBiasThreads;
-    // staggered: the ring this warpgroup signals after issuing a k-block, and the one it waits on
-    uint64_t* const issued_bar = wg == 0 ? lead_bar : follow_bar;
-    uint64_t* const partner_bar = wg == 0 ? follow_bar : lead_bar;
-    float acc[kRB][BN / 2];
+    float acc[BN / 2];
     uint32_t nst = 0;  // TMA stores this warp has issued: picks the staging buffer
-    constexpr int kStep = kPP ? 2 : 1;
-    uint32_t j = 0;  // tiles this warpgroup has taken
-    for (int i = kPP ? wg : 0;; i += kStep, ++j) {
+    for (int i = 0;; ++i) {
       const int tile = blockIdx.x + i * gridDim.x;
       if (tile >= num_tiles) break;
       const int m0 = (tile / num_n) * kBlockM;
       const int n0 = (tile % num_n) * BN;
       if (g.tma_out && g.bias != nullptr) {
-        group_sync<Cfg::kBiasThreads>(1 + bias_group);  // the group's previous epilogue has read the old values
-        stage_bias<BN, Cfg::kBiasThreads>(g, bias_s, n0, bias_tid);
-      }
-      // ping-pong: tile i - 1 (the other warpgroup's) has issued all its wgmmas
-      if (kPP && i > 0) {
-        const long long t0 = tr.now();
-        mbar_wait(&order_bar[wg], (wg == 0 ? j - 1 : j) & 1u);
-        tr.add(kTrOrder, t0);
+        math_sync();  // the previous epilogue has read the old values
+        stage_bias<BN>(g, smem_bias, n0, threadIdx.x - 128);
       }
       uint32_t it = static_cast<uint32_t>(i) * num_kb;  // the ring position of this tile's first k-block
-      const uint32_t it_last = it + num_kb - 1;
       int prev_s = -1;
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const uint32_t s = it % Cfg::kStages;
-        if (kStag && (wg == 1 || it >= kLagMax)) {  // the lag bounds (see the kernel comment)
-          const uint32_t q = wg == 0 ? it - kLagMax : min(it + kLagMin, it_last);
-          const long long t0 = tr.now();
-          mbar_wait(&partner_bar[q % Cfg::kStages], (q / Cfg::kStages) & 1u);
-          tr.add(kTrOrder, t0);
-        }
         const long long t0 = tr.now();
         mbar_wait(&full_bar[s], (it / Cfg::kStages) & 1u);
         if (kb == 0) tr.add(kTrFullFirst, t0);
         else tr.add(kTrFullRest, t0);
-        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + (kPP ? 0 : wg * (64 * 128));
+        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::kStageBytesA) + wg * (64 * 128);
         const uint32_t b_addr = smem_u32(smem_b + s * Cfg::kStageBytesB);
-#pragma unroll
-        for (int rb = 0; rb < kRB; ++rb) wgmma_fence_regs(acc[rb]);
+        wgmma_fence_regs(acc);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
           const uint64_t desc_b = wgmma_desc_sw128(b_addr + k * kWgmmaK * 2);
-#pragma unroll
-          for (int rb = 0; rb < kRB; ++rb)
-            wgmma_ss<BN, kHalfIn>(acc[rb], wgmma_desc_sw128(a_addr + rb * (64 * 128) + k * kWgmmaK * 2), desc_b,
-                                  (kb | k) != 0 ? 1u : 0u);
+          wgmma_ss<BN, kHalfIn>(acc, wgmma_desc_sw128(a_addr + k * kWgmmaK * 2), desc_b, (kb | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
-        if (kPP && kb == num_kb - 1 && lane == 0) mbar_arrive(&order_bar[wg ^ 1]);  // hand the tensor pipe over
-        if (kStag && lane == 0) mbar_arrive(&issued_bar[s]);
         if (prev_s >= 0) {
           const long long t1 = tr.now();
           wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand its shared memory back to the producer
@@ -520,8 +426,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
       }
       long long t0 = tr.now();
       wgmma_wait<0>();
-#pragma unroll
-      for (int rb = 0; rb < kRB; ++rb) wgmma_fence_regs(acc[rb]);
+      wgmma_fence_regs(acc);
       tr.add(kTrWait0, t0);
       if (lane == 0) mbar_arrive(&empty_bar[prev_s]);
       t0 = tr.now();
@@ -529,14 +434,12 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         if (g.bias != nullptr) {
           const long long t1 = tr.now();
           asm volatile("cp.async.wait_all;" ::: "memory");
-          group_sync<Cfg::kBiasThreads>(1 + bias_group);  // every thread's copy has landed
+          math_sync();  // every thread's copy has landed
           tr.add(kTrEpiBias, t1);
         }
-        epilogue_tma<BN, kRB>(g, &tmap_out, acc, bias_s, staging, nst, m0 + warp_row, n0, lane, tr);
+        epilogue_tma<BN>(g, &tmap_out, acc, smem_bias, staging, nst, m0 + warp_row, n0, lane, tr);
       } else {
-#pragma unroll
-        for (int rb = 0; rb < kRB; ++rb)
-          epilogue_direct<BN>(g, acc[rb], m0 + 64 * rb + warp_row + (lane >> 2), n0 + 2 * (lane & 3));
+        epilogue_direct<BN>(g, acc, m0 + warp_row + (lane >> 2), n0 + 2 * (lane & 3));
       }
       tr.add(kTrEpi, t0);
       tr.tick(kTrTiles);
@@ -560,9 +463,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 static unsigned long long* g_trace_buf = nullptr;
 #endif
 
-template <int BN, int kSched, bool kHalfIn>
+template <int BN, bool kHalfIn>
 static int launch_gemm(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, kSched>;
+  using Cfg = GemmCfg<BN>;
   CUtensorMap ta, tw;
   int rc = make_tmap_16bit_2d(&ta, p->a, p->m, p->k, p->lda, kBlockM, kBlockK, kHalfIn);
   if (rc != AB_OK) return rc;
@@ -575,7 +478,7 @@ static int launch_gemm(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, kSched, kHalfIn>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, kHalfIn>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("ab_gemm_bf16: cudaFuncSetAttribute(smem=%d) failed: %s", Cfg::kSmemBytes, cudaGetErrorString(e));
@@ -589,39 +492,74 @@ static int launch_gemm(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
   AB_CHECK_ARG(g_trace_buf != nullptr, "ab_gemm_bf16: traced build without a trace buffer (ab_gemm_trace)");
   args.trace = g_trace_buf;
 #endif
-  gemm_bf16_tn_kernel<BN, kSched, kHalfIn><<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
+  gemm_bf16_tn_kernel<BN, kHalfIn><<<grid, kNumThreads, Cfg::kSmemBytes, stream>>>(ta, tw, tout, args);
   AB_COUNT_LAUNCH(1);
   AB_CHECK_LAUNCH("ab_gemm_bf16");
   return AB_OK;
 }
 
-// The tile shape of each schedule: 128 x 128 per warpgroup for ping-pong, 128 x 256 per CTA for cooperative and
-// staggered while N > 128, 128 x 128 / 128 x 64 cooperative for the narrower decoder heads.
+// 128 x 256 tiles while N > 128, 128 x 128 / 128 x 64 for the narrower decoder heads.
 template <bool kHalfIn>
-static int launch_for(const AbGemm* p, GemmArgs& args, cudaStream_t stream, int sched) {
-  if (p->n > 128) {
-    if (sched == kPingPong) return launch_gemm<128, kPingPong, kHalfIn>(p, args, stream);
-    if (sched == kStaggered) return launch_gemm<256, kStaggered, kHalfIn>(p, args, stream);
-    return launch_gemm<256, kCooperative, kHalfIn>(p, args, stream);
-  }
-  if (p->n > 64) return launch_gemm<128, kCooperative, kHalfIn>(p, args, stream);
-  return launch_gemm<64, kCooperative, kHalfIn>(p, args, stream);
+static int launch_for(const AbGemm* p, GemmArgs& args, cudaStream_t stream) {
+  if (p->n > 128) return launch_gemm<256, kHalfIn>(p, args, stream);
+  if (p->n > 64) return launch_gemm<128, kHalfIn>(p, args, stream);
+  return launch_gemm<64, kHalfIn>(p, args, stream);
 }
 
-// AB_GEMM_SCHEDULE=pingpong|cooperative|staggered, read once: every GEMM with N > 128 takes that schedule instead of
-// the rule in ab_gemm_bf16, so that tools and tests can compare the schedules on the same shapes.  The model never
-// sets it.  -1: unset.
-constexpr int kBadSchedule = -2;
-static int forced_schedule() {
-  static const int forced = [] {
-    const char* e = getenv("AB_GEMM_SCHEDULE");
-    if (e == nullptr || *e == 0) return -1;
-    if (strcmp(e, "pingpong") == 0) return static_cast<int>(kPingPong);
-    if (strcmp(e, "cooperative") == 0) return static_cast<int>(kCooperative);
-    if (strcmp(e, "staggered") == 0) return static_cast<int>(kStaggered);
-    return kBadSchedule;
-  }();
-  return forced;
+// The epilogue's view of p->peer_push (see PeerRows): one row range per level and side, and the number of boxes that
+// carry peer rows, into a zeroed pr.  tma_out: the launch takes the 16-bit-only epilogue, the one that pushes.
+static int peer_rows(const AbGemm* p, int tma_out, PeerRows& pr) {
+  const AbHaloPush* h = p->peer_push;
+  AB_CHECK_ARG(tma_out && p->out_dtype == AB_DT_BF16, "ab_gemm_bf16: peer_push needs a 16-bit-only bf16 output");
+  AB_CHECK_ARG(h->c > 0 && 2 * h->c <= 8 && static_cast<long long>(h->c) * h->rows * h->w == p->m &&
+                   h->src_tok_bytes == 2ll * p->n && h->tok_off_bytes % 128 == 0 &&
+                   h->tok_off_bytes + h->tok_bytes == h->src_tok_bytes && h->rows_to_above <= h->rows &&
+                   h->rows_to_below <= h->rows && h->rows_to_above <= h->slot_rows && h->rows_to_below <= h->slot_rows,
+               "ab_gemm_bf16: peer_push does not describe this output (c=%d rows=%d w=%d, m=%d n=%d)", h->c, h->rows,
+               h->w, p->m, p->n);
+  pr.col_from = static_cast<int>(h->tok_off_bytes / 2);
+  pr.dst_ld = static_cast<int>(h->tok_bytes / 2);
+  pr.flag[0] = h->above_flag;
+  pr.flag[1] = h->below_flag;
+  pr.ctrl = h->ctrl;
+  const long long slot_row_elems = static_cast<long long>(h->w) * pr.dst_ld;
+  for (int c = 0; c < h->c; ++c) {
+    if (h->rows_to_above > 0) {  // my first rows -> rows [0, n) of the slot of the rank above
+      const int i = pr.n_ranges++;
+      pr.row_begin[i] = (c * h->rows) * h->w;
+      pr.row_end[i] = pr.row_begin[i] + h->rows_to_above * h->w;
+      pr.dst[i] = reinterpret_cast<uint16_t*>(h->above_slot) + static_cast<long long>(c) * h->slot_rows * slot_row_elems;
+    }
+    if (h->rows_to_below > 0) {  // my last rows -> rows [slot_rows - n, slot_rows) of the slot of the rank below
+      const int i = pr.n_ranges++;
+      pr.row_begin[i] = (c * h->rows + h->rows - h->rows_to_below) * h->w;
+      pr.row_end[i] = pr.row_begin[i] + h->rows_to_below * h->w;
+      pr.dst[i] = reinterpret_cast<uint16_t*>(h->below_slot) +
+                  (static_cast<long long>(c) * h->slot_rows + h->slot_rows - h->rows_to_below) * slot_row_elems;
+    }
+  }
+  AB_CHECK_ARG(pr.n_ranges > 0, "ab_gemm_bf16: peer_push with nothing to send (use ab_halo_push, which still publishes)");
+  // boxes of this launch that carry peer rows: distinct 16-row groups touched by any range x 64-column boxes sent.
+  // Ranges are emitted in increasing row order per level, and levels increase: a sweep over sorted begins suffices.
+  int order[8];
+  for (int i = 0; i < pr.n_ranges; ++i) order[i] = i;
+  for (int i = 1; i < pr.n_ranges; ++i)
+    for (int j = i; j > 0 && pr.row_begin[order[j]] < pr.row_begin[order[j - 1]]; --j) {
+      const int t = order[j];
+      order[j] = order[j - 1];
+      order[j - 1] = t;
+    }
+  int groups = 0, last_group = -1;
+  for (int k = 0; k < pr.n_ranges; ++k) {
+    const int i = order[k];
+    int g0 = pr.row_begin[i] / kBoxRows;
+    const int g1 = (pr.row_end[i] - 1) / kBoxRows;
+    if (g0 <= last_group) g0 = last_group + 1;
+    if (g1 >= g0) groups += g1 - g0 + 1;
+    if (g1 > last_group) last_group = g1;
+  }
+  pr.expected = groups * ((p->n - pr.col_from + 63) / 64);
+  return AB_OK;
 }
 
 #ifdef AB_GEMM_TRACE
@@ -675,72 +613,10 @@ extern "C" int ab_gemm_bf16(const AbGemm* p, void* stream) {
   a.tma_out = p->out_bf16 != nullptr && p->out_f32 == nullptr && p->residual == nullptr && al16(p->out_bf16) &&
               p->ld_bf16 % 8 == 0 && (p->bias == nullptr || (reinterpret_cast<uintptr_t>(p->bias) & 15u) == 0);
   if (p->peer_push != nullptr) {
-    const AbHaloPush* h = p->peer_push;
-    AB_CHECK_ARG(a.tma_out && p->out_dtype == AB_DT_BF16, "ab_gemm_bf16: peer_push needs a 16-bit-only bf16 output");
-    AB_CHECK_ARG(h->c > 0 && 2 * h->c <= 8 && static_cast<long long>(h->c) * h->rows * h->w == p->m &&
-                     h->src_tok_bytes == 2ll * p->n && h->tok_off_bytes % 128 == 0 &&
-                     h->tok_off_bytes + h->tok_bytes == h->src_tok_bytes && h->rows_to_above <= h->rows &&
-                     h->rows_to_below <= h->rows && h->rows_to_above <= h->slot_rows && h->rows_to_below <= h->slot_rows,
-                 "ab_gemm_bf16: peer_push does not describe this output (c=%d rows=%d w=%d, m=%d n=%d)", h->c, h->rows,
-                 h->w, p->m, p->n);
-    PeerRows& pr = a.peer;
-    pr.col_from = static_cast<int>(h->tok_off_bytes / 2);
-    pr.dst_ld = static_cast<int>(h->tok_bytes / 2);
-    pr.flag[0] = h->above_flag;
-    pr.flag[1] = h->below_flag;
-    pr.ctrl = h->ctrl;
-    const long long slot_row_elems = static_cast<long long>(h->w) * pr.dst_ld;
-    for (int c = 0; c < h->c; ++c) {
-      if (h->rows_to_above > 0) {  // my first rows -> rows [0, n) of the slot of the rank above
-        const int i = pr.n_ranges++;
-        pr.row_begin[i] = (c * h->rows) * h->w;
-        pr.row_end[i] = pr.row_begin[i] + h->rows_to_above * h->w;
-        pr.dst[i] = reinterpret_cast<uint16_t*>(h->above_slot) + static_cast<long long>(c) * h->slot_rows * slot_row_elems;
-      }
-      if (h->rows_to_below > 0) {  // my last rows -> rows [slot_rows - n, slot_rows) of the slot of the rank below
-        const int i = pr.n_ranges++;
-        pr.row_begin[i] = (c * h->rows + h->rows - h->rows_to_below) * h->w;
-        pr.row_end[i] = pr.row_begin[i] + h->rows_to_below * h->w;
-        pr.dst[i] = reinterpret_cast<uint16_t*>(h->below_slot) +
-                    (static_cast<long long>(c) * h->slot_rows + h->slot_rows - h->rows_to_below) * slot_row_elems;
-      }
-    }
-    AB_CHECK_ARG(pr.n_ranges > 0, "ab_gemm_bf16: peer_push with nothing to send (use ab_halo_push, which still publishes)");
-    // boxes of this launch that carry peer rows: distinct 16-row groups touched by any range x 64-column boxes sent
-    int groups = 0, last_group = -1;
-    for (int pass = 0; pass < 1; ++pass) {
-      // ranges are emitted in increasing row order per level, and levels increase: a sweep over sorted begins suffices
-      int order[8];
-      for (int i = 0; i < pr.n_ranges; ++i) order[i] = i;
-      for (int i = 1; i < pr.n_ranges; ++i)
-        for (int j = i; j > 0 && pr.row_begin[order[j]] < pr.row_begin[order[j - 1]]; --j) {
-          const int t = order[j];
-          order[j] = order[j - 1];
-          order[j - 1] = t;
-        }
-      for (int k = 0; k < pr.n_ranges; ++k) {
-        const int i = order[k];
-        int g0 = pr.row_begin[i] / kBoxRows;
-        const int g1 = (pr.row_end[i] - 1) / kBoxRows;
-        if (g0 <= last_group) g0 = last_group + 1;
-        if (g1 >= g0) groups += g1 - g0 + 1;
-        if (g1 > last_group) last_group = g1;
-      }
-    }
-    pr.expected = groups * ((p->n - pr.col_from + 63) / 64);
+    const int rc = peer_rows(p, a.tma_out, a.peer);
+    if (rc != AB_OK) return rc;
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  // Every shape takes the cooperative tile (128 x 256 for N > 128).  Since the epilogue no longer waits on global loads
-  // or on its stores (3.3 us per 128 x 256 tile, 4.9-5.3 us with GELU), the cooperative main loop, whose wgmmas read
-  // fewer shared-memory bytes per FLOP (48 KB of operands per 128 x 256 x 64 step against 32 KB per 128 x 128 x 64),
-  // costs less than the ping-pong tile's hidden epilogue saves: with every shape cooperative the 0.25-degree step ran
-  // 3 % faster than with ping-pong at K <= 1024, and ping-pong at K <= 1024 for N <= 1024 only was no better (DESIGN
-  // §6).  Staggered loses to both: its lag waits cost more than the epilogue time it hides.  Both stay for
-  // AB_GEMM_SCHEDULE.
-  int sched = kCooperative;
-  const int forced = forced_schedule();
-  AB_CHECK_ARG(forced != kBadSchedule, "ab_gemm_bf16: AB_GEMM_SCHEDULE must be pingpong, cooperative or staggered");
-  if (forced >= 0 && p->n > 128) sched = forced;
-  if (p->in_dtype == AB_DT_F16) return launch_for<true>(p, a, s, sched);
-  return launch_for<false>(p, a, s, sched);
+  if (p->in_dtype == AB_DT_F16) return launch_for<true>(p, a, s);
+  return launch_for<false>(p, a, s);
 }

@@ -565,11 +565,11 @@ def test_unpatchify_modulation_and_clamps_keep_nan():
 # GEMM epilogues with 16-bit (fp16 / bf16) outputs
 # ------------------------------------------------------------------------------------------------
 GEMM_CASES = {  # (m, n, k, epilogue)
-    "tma_pingpong": (300, 264, 256, "tma"),        # N > 128, K <= 1024: ping-pong 128 x 128 tiles
-    "tma_coop256": (300, 264, 1088, "tma"),        # K > 1024: cooperative 128 x 256
-    "tma_coop128": (200, 96, 128, "tma"),          # N <= 128: cooperative 128 x 128
+    "tma_coop256_k256": (300, 264, 256, "tma"),    # N > 128: 128 x 256 tiles, 8 live columns in the second
+    "tma_coop256": (300, 264, 1088, "tma"),        # 128 x 256, K tail past 1024
+    "tma_coop128": (200, 96, 128, "tma"),          # N <= 128: 128 x 128
     "direct_dual": (300, 131, 256, "dual"),        # fp32 + 16-bit outputs, residual: direct epilogue (odd N: to16 tail)
-    "direct_dual_pingpong_shape": (257, 520, 512, "dual"),
+    "direct_dual_coop256": (257, 520, 512, "dual"),  # direct epilogue on 128 x 256 tiles, 8 live columns in the third
     "direct_unaligned": (200, 200, 128, "unaligned"),  # 16-bit output 2 bytes off 16-byte alignment: scalar stores
 }
 

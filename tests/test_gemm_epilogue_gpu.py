@@ -51,11 +51,11 @@ def _check(m, n, k, dtype, gelu, bias=True, pad=0, seed=0):
 
 
 @pytest.mark.parametrize("m,n,k", [
-    (300, 131, 256),    # ping-pong 128 x 128: 3 live columns in the second tile
-    (1000, 1029, 512),  # ping-pong: 5 live columns in the last tile, 1 in its last group of 8
-    (257, 190, 1024),   # ping-pong: N tail inside the second 64-column box, 62 = 7 groups of 8 + 6
-    (500, 303, 1088),   # cooperative 128 x 256 (K > 1024): 47 live columns in the second tile
-    (333, 83, 136),     # cooperative 128 x 128: 19 live columns in the second 64-column box
+    (300, 131, 256),    # 128 x 256: 3 live columns in the third 64-column box
+    (1000, 1029, 512),  # 128 x 256: 5 live columns in the last tile
+    (257, 190, 1024),   # 128 x 256: N tail inside the third 64-column box, 62 = 7 groups of 8 + 6
+    (500, 303, 1088),   # 128 x 256, K tail past 1024: 47 live columns in the second tile
+    (333, 83, 136),     # 128 x 128: 19 live columns in the second 64-column box
     (141, 61, 64),      # the 64-wide tile: 61 of 64 columns
 ])
 @pytest.mark.parametrize("gelu", [False, True], ids=["bias", "bias_gelu"])

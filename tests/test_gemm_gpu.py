@@ -63,7 +63,7 @@ def test_gemm_matches_fp32_reference(m, n, k, mode):
     torch.testing.assert_close(out_bf16.float(), ref, rtol=1e-2, atol=1e-2)
 
 
-WIDE_SHAPES = [
+LONG_K_SHAPES = [
     (1024, 256, 1024),    # eight full 128-row tiles
     (1500, 520, 1024),    # M tail inside the second warpgroup's rows, N tail (8 live columns in the last block)
     (2049, 256, 1088),    # one row into a new tile (all but one 16-row box fully out of bounds), odd k-block count
@@ -72,12 +72,11 @@ WIDE_SHAPES = [
 ]
 
 
-@pytest.mark.parametrize("m,n,k", WIDE_SHAPES)
+@pytest.mark.parametrize("m,n,k", LONG_K_SHAPES)
 @pytest.mark.parametrize("mode", ["plain_bf16", "bias_gelu_bf16", "bias_res_f32_dual"])
-def test_wide_pair_kernel_matches_reference_and_pair_kernel(m, n, k, mode, monkeypatch):
+def test_long_k_matches_reference_and_repeats_bit_identically(m, n, k, mode):
     """Large shapes with K >= 1024 (long main loops, many tiles per CTA): fp32 reference tolerance, and two launches on
-    the same operands are bit-identical (the persistent schedule fixes the fp32 accumulation order over K).  The name
-    dates from a kernel family that had a separate wide-tile variant for these shapes."""
+    the same operands are bit-identical (the persistent schedule fixes the fp32 accumulation order over K)."""
     from aurora_b200 import cabi
 
     torch.manual_seed(m + n + k)
@@ -87,20 +86,20 @@ def test_wide_pair_kernel_matches_reference_and_pair_kernel(m, n, k, mode, monke
     bias = torch.randn(n, device=dev) if mode != "plain_bf16" else None
     residual = torch.randn(m, n, device=dev) if mode == "bias_res_f32_dual" else None
     act = cabi.AB_ACT_GELU_ERF if mode == "bias_gelu_bf16" else cabi.AB_ACT_NONE
-    outs = {}
-    for wide in ("2", "0"):  # first and second launch
+    outs = []
+    for _ in range(2):
         out_bf16 = torch.full((m, n), float("nan"), device=dev, dtype=torch.bfloat16)
         out_f32 = torch.full((m, n), float("nan"), device=dev) if mode == "bias_res_f32_dual" else None
         cabi.gemm(a, w, bias=bias, residual=residual, out_f32=out_f32, out_bf16=out_bf16, act=act)
         torch.cuda.synchronize()
-        outs[wide] = (out_bf16, out_f32)
+        outs.append((out_bf16, out_f32))
     ref = _ref(a, w, bias, residual, act)
-    out_bf16, out_f32 = outs["2"]
+    (out_bf16, out_f32), (again_bf16, again_f32) = outs
     if out_f32 is not None:
         torch.testing.assert_close(out_f32, ref, rtol=1e-4, atol=1e-4)
-        assert torch.equal(out_f32, outs["0"][1])
+        assert torch.equal(out_f32, again_f32)
     torch.testing.assert_close(out_bf16.float(), ref, rtol=1e-2, atol=1e-2)
-    assert torch.equal(out_bf16, outs["0"][0])
+    assert torch.equal(out_bf16, again_bf16)
 
 
 def test_gemm_strided_views():
@@ -197,20 +196,17 @@ def test_gemm_ln_residual_rejects_other_widths():
 # ------------------------------------------------------------------------------------------------------------
 # fused compute + exchange: the epilogue also stores boundary rows into (peer) halo slots (AbGemm.peer_push)
 # ------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("variant", ["single", "pair", "wide"])
+@pytest.mark.parametrize("rows,w", [(5, 12), (10, 36), (30, 144)])
 @pytest.mark.parametrize("to_above,to_below", [(3, 2), (0, 5), (1, 0)])
-def test_gemm_epilogue_pushes_boundary_rows_into_halo_slots(variant, to_above, to_below, monkeypatch):
+def test_gemm_epilogue_pushes_boundary_rows_into_halo_slots(rows, w, to_above, to_below):
     """The QKV projection of a latitude band [C, rows, W, 3D] with `peer_push`: columns [D, 3D) of the first `to_above`
     and last `to_below` rows of every level land in the halo slots (here: in this GPU's own memory) exactly as
     `ab_halo_push` would place them, the round is published in both flags once, the completion counter is back at zero,
-    and the regular output is untouched by the extra stores.  "single": fewer tiles than SMs; "pair" / "wide": the
-    full-size band, several tiles per CTA (the names date from a kernel family with one variant per size class)."""
+    and the regular output is untouched by the extra stores.  M = 240, 1440 and 17280: 6 and 36 tiles of 128 x 256,
+    fewer than SMs, and 405 tiles, several per CTA."""
     from aurora_b200 import cabi
 
-    c, rows, w, d, k, slot_rows = 4, 10, 36, 256, 1024, 5
-    if variant == "single":
-        rows, w = 5, 12          # M = 240: two row tiles
-        to_above, to_below = min(to_above, rows), min(to_below, rows)
+    c, d, k, slot_rows = 4, 256, 1024, 5
     m, n = c * rows * w, 3 * d
     torch.manual_seed(c + rows + w + to_above)
     dev = "cuda"

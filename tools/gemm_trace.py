@@ -12,16 +12,16 @@
      tile_us          CTA time over the tiles the CTA ran
      producer         empty_bar waits of the TMA producer
      full_first       full_bar wait of a tile's first k-block    |
-     full_rest        full_bar waits of its other k-blocks        |
-     order            order_bar wait (ping-pong), lag waits       |  per math warp, over the tiles
-                      (staggered)                                 |
+     full_rest        full_bar waits of its other k-blocks        |  per math warp, over the tiles
      wait1 / wait0    wgmma_wait<1> / <0>                         |  that warp's warpgroup took
      epilogue         the whole epilogue, of which                |
        store_wait     waits for a store buffer                    |
        bias_wait      waits for the bias values                   |
        math_store     the rest: bias, GELU, packing, stores       |
    plus the card line (name, power limit, max SM clock) from the same run.
-   AB_GEMM_SCHEDULE=pingpong|cooperative|staggered in the environment traces that schedule (N > 128 shapes).
+
+A `--source` whose trace record has other slots than these (a gemm.cu up to f9f866b, with the `order` slot of
+the ping-pong and staggered schedules) fails the record-size assert instead of being misread.
 
 Writes build/trace/ only; needs a GPU to run.
 """
@@ -60,7 +60,7 @@ SHAPES = [
 ]
 
 CTA_WORDS = 6  # timer start / end, clock start / end, producer empty waits, producer tiles
-SLOTS = ["full_first", "full_rest", "order", "wait1", "wait0", "epilogue", "store_wait", "bias_wait", "tiles"]
+SLOTS = ["full_first", "full_rest", "wait1", "wait0", "epilogue", "store_wait", "bias_wait", "tiles"]
 
 
 def build_libs(source: Path) -> tuple[Path, Path]:
