@@ -1,6 +1,6 @@
 """aurora_b200 — Hopper (H100, sm_90a) implementation of Aurora's forward pass behind the reference's API
 (`aurora/__init__.py:3-30`): ``Aurora*`` model classes, ``Batch``, ``Metadata``, ``rollout`` and ``Tracker``,
-plus ``Scorer``, which scores predictions against an analysis on the GPU."""
+plus ``Scorer`` and ``EnsembleScorer``, which score predictions and ensembles against an analysis on the GPU."""
 
 from aurora_b200.batch import Batch, Metadata
 from aurora_b200.model import (
@@ -14,11 +14,11 @@ from aurora_b200.model import (
     AuroraWave,
 )
 from aurora_b200.rollout import rollout
-from aurora_b200.scorer import Scorer
+from aurora_b200.scorer import EnsembleScorer, Scorer
 from aurora_b200.tracker import Tracker
 
 __all__ = [
     "Aurora", "AuroraPretrained", "AuroraSmallPretrained", "AuroraSmall", "Aurora12hPretrained", "AuroraHighRes",
     "AuroraAirPollution", "AuroraWave", "Batch", "Metadata", "rollout",
-    "Tracker", "Scorer",
+    "Tracker", "Scorer", "EnsembleScorer",
 ]

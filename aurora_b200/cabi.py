@@ -20,6 +20,7 @@ __all__ = [
     "linear_small", "patchify", "unpatchify", "AbFieldIn", "AbFieldOut", "ipc_export", "ipc_open", "ipc_close",
     "halo_push", "halo_wait", "AbSwinBlock", "swin_block", "swin_block_workspace_bytes", "gemm_ln_supported",
     "gemm_ln_residual", "AbTrackBox", "track_boxes", "AbScoreField", "score_workspace_bytes", "score_fields",
+    "AbEnsembleField", "ensemble_score_workspace_bytes", "ensemble_score_fields",
 ]
 
 ABI_VERSION = 2  # == AB_ABI_VERSION in include/aurora_b200.h
@@ -119,6 +120,8 @@ EXPORTS = [
     "ab_track_boxes",
     "ab_score_workspace_bytes",
     "ab_score_fields",
+    "ab_ensemble_score_workspace_bytes",
+    "ab_ensemble_score_fields",
 ]
 AB_IPC_HANDLE_BYTES = 64
 AB_HALO_CTRL_BYTES = 256
@@ -735,3 +738,41 @@ def score_fields(fields: list, row_weights: torch.Tensor, sums: torch.Tensor, wo
     check(lib().ab_score_fields(arr, len(fields), C.c_size_t(C.sizeof(AbScoreField)), C.c_void_p(ptr(row_weights)),
                                 C.c_void_p(ptr(sums)), C.c_void_p(ptr(workspace)), C.c_size_t(nbytes), _s()),
           "ab_score_fields")
+
+
+AB_ENS_MAX_MEMBERS = 64
+AB_ENS_MAX_FIELDS = 16
+# W, sum w (xm - y), sum w (xm - y)^2, sum w s^2, sum w crps skill, sum w crps spread, sum w af ao, sum w af^2,
+# sum w ao^2, count
+AB_ENS_SUMS = 10
+
+
+class AbEnsembleField(C.Structure):
+    _fields_ = [
+        ("members", C.c_void_p * AB_ENS_MAX_MEMBERS), ("truth", C.c_void_p), ("clim", C.c_void_p),
+        ("member_level_stride", C.c_int64), ("truth_level_stride", C.c_int64), ("clim_level_stride", C.c_int64),
+        ("n_members", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+        ("ld_member", C.c_int32), ("ld_truth", C.c_int32), ("ld_clim", C.c_int32),
+        ("levels", C.c_int32),
+    ]
+
+
+def ensemble_score_workspace_bytes(fields: list) -> int:
+    arr = (AbEnsembleField * max(len(fields), 1))(*fields)
+    n = C.c_size_t()
+    check(lib().ab_ensemble_score_workspace_bytes(arr, len(fields), C.c_size_t(C.sizeof(AbEnsembleField)),
+                                                  C.byref(n)), "ab_ensemble_score_workspace_bytes")
+    return int(n.value)
+
+
+def ensemble_score_fields(fields: list, row_weights: torch.Tensor, sums: torch.Tensor,
+                          workspace: torch.Tensor) -> None:
+    """One call over `fields` (`AbEnsembleField` list): `row_weights` float64 [h], `sums` float64 [planes, 10] (a view
+    with contiguous rows), `workspace` of at least `ensemble_score_workspace_bytes(fields)` bytes, all on the device."""
+    assert row_weights.dtype == torch.float64 and sums.dtype == torch.float64 and sums.is_contiguous()
+    arr = (AbEnsembleField * max(len(fields), 1))(*fields)
+    nbytes = workspace.numel() * workspace.element_size()
+    check(lib().ab_ensemble_score_fields(arr, len(fields), C.c_size_t(C.sizeof(AbEnsembleField)),
+                                         C.c_void_p(ptr(row_weights)), C.c_void_p(ptr(sums)),
+                                         C.c_void_p(ptr(workspace)), C.c_size_t(nbytes), _s()),
+          "ab_ensemble_score_fields")

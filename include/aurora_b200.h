@@ -498,6 +498,51 @@ int ab_score_workspace_bytes(const AbScoreField* fields, int32_t n_fields, size_
 int ab_score_fields(const AbScoreField* fields, int32_t n_fields, size_t field_bytes, const double* row_weights,
                     double* sums, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Latitude-weighted scores of a device-resident ensemble against a truth (and a climatology): the sums behind the
+ * ensemble-mean RMSE and bias, the spread, the fair CRPS and the ensemble-mean ACC, for every level plane of every
+ * field, in one call.  Not a reference function.
+ *
+ * One AbEnsembleField per variable: n_members (2 <= M <= AB_ENS_MAX_MEMBERS) member pointers that share one row pitch
+ * ld_member and one level stride, a truth and a clim (may be NULL), each `levels` planes of h x w float32 values.
+ * Planes are numbered field by field, level by level.  For plane p, with w_r = row_weights[r] (double [h] of the
+ * largest h, DEVICE memory), a point valid when the truth, every member and (if given) clim are all not NaN, x_k the
+ * member values, xm their mean, s2 their unbiased variance (all in double), y = truth and c = clim,
+ * sums[p][0..9] =
+ *   W = sum w_r,  sum w_r (xm - y),  sum w_r (xm - y)^2,  sum w_r s2,  sum w_r (1/M) sum_k |x_k - y|,
+ *   sum w_r (1/(M(M-1))) sum_{k != l} |x_k - x_l|,  sum w_r af ao,  sum w_r af^2,  sum w_r ao^2,  count,
+ * over the valid points, af = xm - c, ao = y - c; sums 6..8 are 0 without clim.  +-inf is not skipped.  Each point's
+ * member values are sorted (a bitonic network over 8, 16, 32 or 64 values, the smallest that holds the largest M of
+ * the call) and every per-point quantity is formed in that order, so the sums do not depend on the order of the
+ * members, bit for bit.  Rows are split into a fixed (plane, row-chunk) partition whose partial sums go to
+ * `workspace` and are added in a fixed order by a second launch, so repeated calls give bit-identical sums (no
+ * atomics).  `fields` is a HOST array copied into the launch; `field_bytes` must be sizeof(AbEnsembleField);
+ * 0 <= n_fields <= AB_ENS_MAX_FIELDS (0 is a no-op); h, w, levels >= 1, ld_* >= w, level strides >= 0; 16-byte loads
+ * where every pointer, pitch, level stride and the width of a field allow, scalar loads otherwise.  `sums` is
+ * double [total planes][AB_ENS_SUMS], DEVICE memory.
+ * ---------------------------------------------------------------------------------------------- */
+#define AB_ENS_MAX_MEMBERS 64
+#define AB_ENS_MAX_FIELDS 16 /* the 9 variables of the 1.3 B model in one call; the launch parameter is ~9.6 KB */
+#define AB_ENS_SUMS 10
+
+typedef struct AbEnsembleField {
+  const float* members[AB_ENS_MAX_MEMBERS]; /* the first n_members: f32 [levels][h, ld_member] each */
+  const float* truth;                       /* f32 [levels][h, ld_truth] */
+  const float* clim;                        /* f32 [levels][h, ld_clim] or NULL */
+  int64_t member_level_stride, truth_level_stride, clim_level_stride; /* elements between consecutive levels */
+  int32_t n_members;
+  int32_t h, w;
+  int32_t ld_member, ld_truth, ld_clim;
+  int32_t levels;
+} AbEnsembleField;
+
+/* Workspace `ab_ensemble_score_fields` needs for these fields (validates them like it does).  Host only. */
+int ab_ensemble_score_workspace_bytes(const AbEnsembleField* fields, int32_t n_fields, size_t field_bytes,
+                                      size_t* bytes);
+int ab_ensemble_score_fields(const AbEnsembleField* fields, int32_t n_fields, size_t field_bytes,
+                             const double* row_weights, double* sums, void* workspace, size_t workspace_bytes,
+                             void* stream);
+
 /* sizeof() of the descriptor structs as this library was compiled (binding authors: compare with your mirror).
  * which: 0 AbGemm, 1 AbWindowAttention, 2 AbLnModResidual, 3 AbFieldIn, 4 AbFieldOut, 5 AbHaloPush, 6 AbSwinBlock,
  * 7 AbGemmLn, 8 AbPatchMergeLn, 9 AbPatchSplitLn, 10 AbOp; -1 for an unknown index.  Host only. */
