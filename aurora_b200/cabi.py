@@ -20,7 +20,8 @@ __all__ = [
     "linear_small", "patchify", "unpatchify", "AbFieldIn", "AbFieldOut", "ipc_export", "ipc_open", "ipc_close",
     "halo_push", "halo_wait", "AbSwinBlock", "swin_block", "swin_block_workspace_bytes", "gemm_ln_supported",
     "gemm_ln_residual", "AbTrackBox", "track_boxes", "AbScoreField", "score_workspace_bytes", "score_fields",
-    "AbEnsembleField", "ensemble_score_workspace_bytes", "ensemble_score_fields",
+    "AbEnsembleField", "ensemble_score_workspace_bytes", "ensemble_score_fields", "AbSpectrumField",
+    "zonal_spectra_workspace_bytes", "zonal_spectra",
 ]
 
 ABI_VERSION = 2  # == AB_ABI_VERSION in include/aurora_b200.h
@@ -122,6 +123,8 @@ EXPORTS = [
     "ab_score_fields",
     "ab_ensemble_score_workspace_bytes",
     "ab_ensemble_score_fields",
+    "ab_zonal_spectra_workspace_bytes",
+    "ab_zonal_spectra",
 ]
 AB_IPC_HANDLE_BYTES = 64
 AB_HALO_CTRL_BYTES = 256
@@ -776,3 +779,44 @@ def ensemble_score_fields(fields: list, row_weights: torch.Tensor, sums: torch.T
                                          C.c_void_p(ptr(row_weights)), C.c_void_p(ptr(sums)),
                                          C.c_void_p(ptr(workspace)), C.c_size_t(nbytes), _s()),
           "ab_ensemble_score_fields")
+
+
+# ---- latitude-band zonal power spectra (csrc/spectra.cu) ------------------------------------------------------------
+AB_SPEC_MAX_FIELDS = 64
+AB_SPEC_MAX_BANDS = 8
+AB_SPEC_MAX_WIDTH = 4096
+
+
+class AbSpectrumField(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("level_stride", C.c_int64),
+        ("h", C.c_int32), ("w", C.c_int32), ("ld", C.c_int32), ("levels", C.c_int32),
+    ]
+
+
+def _band_rows(bands: list) -> C.Array:
+    return (C.c_int32 * (2 * max(len(bands), 1)))(*(r for band in bands for r in band))
+
+
+def zonal_spectra_workspace_bytes(fields: list, bands: list) -> int:
+    """`bands`: [(r0, r1)] row ranges."""
+    arr = (AbSpectrumField * max(len(fields), 1))(*fields)
+    n = C.c_size_t()
+    check(lib().ab_zonal_spectra_workspace_bytes(arr, len(fields), C.c_size_t(C.sizeof(AbSpectrumField)),
+                                                 _band_rows(bands), len(bands), C.byref(n)),
+          "ab_zonal_spectra_workspace_bytes")
+    return int(n.value)
+
+
+def zonal_spectra(fields: list, bands: list, row_weights: torch.Tensor, out: torch.Tensor,
+                  workspace: torch.Tensor) -> None:
+    """One call over `fields` (`AbSpectrumField` list of one grid) and `bands` ([(r0, r1)] row ranges): `row_weights`
+    float64 [h], `out` float64 [planes, n_bands * (w // 2 + 3)] (a view with contiguous rows), `workspace` of at least
+    `zonal_spectra_workspace_bytes(fields, bands)` bytes, all on the device."""
+    assert row_weights.dtype == torch.float64 and out.dtype == torch.float64 and out.is_contiguous()
+    arr = (AbSpectrumField * max(len(fields), 1))(*fields)
+    nbytes = workspace.numel() * workspace.element_size()
+    check(lib().ab_zonal_spectra(arr, len(fields), C.c_size_t(C.sizeof(AbSpectrumField)), _band_rows(bands),
+                                 len(bands), C.c_void_p(ptr(row_weights)), C.c_void_p(ptr(out)),
+                                 C.c_void_p(ptr(workspace)), C.c_size_t(nbytes), _s()),
+          "ab_zonal_spectra")

@@ -11,7 +11,7 @@
 // give bit-identical sums.
 #include <math.h>
 
-#include "common.h"
+#include "score.cuh"
 
 namespace ab {
 namespace {
@@ -342,21 +342,6 @@ __global__ void __launch_bounds__(kThreads) ens_partial_kernel(const __grid_cons
 }
 
 // ---- host side --------------------------------------------------------------------------------------------------
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
-// The checks both entry points make on the descriptor array itself.
-int check_array(const void* fields, int32_t n_fields, size_t field_bytes, size_t want, const char* type,
-                int max_fields, const char* who) {
-  AB_CHECK_ARG(field_bytes == want, "%s: field_bytes %zu != sizeof(%s) %zu", who, field_bytes, type, want);
-  AB_CHECK_ARG(n_fields >= 0, "%s: n_fields %d < 0", who, n_fields);
-  if (n_fields > max_fields) {
-    set_error("%s: %d fields in one call, at most %d are supported", who, n_fields, max_fields);
-    return AB_ERR_UNSUPPORTED;
-  }
-  AB_CHECK_ARG(n_fields == 0 || fields, "%s: null argument", who);
-  return AB_OK;
-}
-
 // Field i of the partition: whole rows, about `points` points per work item.
 template <int kMaxFields>
 int add_field(Partition<kMaxFields>* p, int i, int h, int w, int levels, int points, int64_t* items,

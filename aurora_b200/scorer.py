@@ -97,9 +97,9 @@ def _ensemble_field(members: list[torch.Tensor], truth: torch.Tensor,
 
 
 class _StepScorer:
-    """What `Scorer` and `EnsembleScorer` share: the climatology and variable selection, the checks of a truth or
-    climatology against a prediction, host copies of coordinates, row weights and the device sums, `_SUMS` per plane,
-    that `step` appends to."""
+    """What `Scorer`, `EnsembleScorer` and `ZonalSpectra` share: the climatology and variable selection, the checks of
+    a truth or climatology against a prediction, host copies of coordinates, row weights and the device sums that
+    `step` appends to: one row per plane, `_SUMS` values wide unless a call says otherwise, packed end to end."""
 
     _SUMS = cabi.AB_SCORE_SUMS
 
@@ -107,7 +107,8 @@ class _StepScorer:
         self.climatology = climatology
         self.variables = None if variables is None else tuple(variables)
         self._rows: list[tuple] = []  # one per plane
-        self._sums: Optional[torch.Tensor] = None  # float64 [capacity, _SUMS] on the predictions' device
+        self._sums: Optional[torch.Tensor] = None  # float64 [capacity] on the predictions' device
+        self._used = 0  # values of `_sums` the rows fill
         self._workspace: Optional[torch.Tensor] = None
         self._host: dict[int, tuple[torch.Tensor, np.ndarray]] = {}  # coordinate tensors seen, by identity
         self._weights: dict[tuple, torch.Tensor] = {}
@@ -181,19 +182,21 @@ class _StepScorer:
                                  f"{lat.size} x {md.lon.numel()}")
         return sizes.pop(), [levels.index(lv) for lv in md.atmos_levels if lv in levels]
 
-    def _append(self, n: int, device: torch.device) -> torch.Tensor:
-        """`n` fresh rows at the end of the device sums (grown by copying on the device, never read back)."""
-        used = len(self._rows)
+    def _append(self, n: int, device: torch.device, width: int) -> torch.Tensor:
+        """`n` fresh rows of `width` values at the end of the device sums (grown by copying on the device, never read
+        back), as an [n, width] view."""
+        used = self._used
         if self._sums is not None and self._sums.device != device:
             raise ValueError(f"{type(self).__name__} holds scores on {self._sums.device}; "
                              f"the prediction is on {device}")
-        if self._sums is None or self._sums.shape[0] < used + n:
-            cap = max(used + n, 256, 0 if self._sums is None else 2 * self._sums.shape[0])
-            grown = torch.empty(cap, self._SUMS, dtype=torch.float64, device=device)
+        need = used + n * width
+        if self._sums is None or self._sums.numel() < need:
+            cap = max(need, 256 * self._SUMS, 0 if self._sums is None else 2 * self._sums.numel())
+            grown = torch.empty(cap, dtype=torch.float64, device=device)
             if used:
                 grown[:used].copy_(self._sums[:used])
             self._sums = grown
-        return self._sums[used:used + n]
+        return self._sums[used:need].view(n, width)
 
     def _check_prediction(self, pred: Batch, what: str = "prediction") -> None:
         """Refuse a sharded or 2-D-coordinate prediction."""
@@ -227,9 +230,11 @@ class _StepScorer:
         return truth, clim
 
     def _score(self, fields: list, rows: list, weights: torch.Tensor, device: torch.device, max_fields: int,
-               workspace_bytes, score) -> None:
-        """Score `fields` in calls of at most `max_fields` into fresh rows of the device sums."""
-        sums = self._append(len(rows), device)
+               workspace_bytes, score, width: Optional[int] = None) -> None:
+        """Score `fields` in calls of at most `max_fields` into fresh rows (one per plane, `width` values, by default
+        `_SUMS`) of the device sums."""
+        width = self._SUMS if width is None else width
+        sums = self._append(len(rows), device, width)
         done = 0
         for s0 in range(0, len(fields), max_fields):
             chunk = fields[s0:s0 + max_fields]
@@ -240,10 +245,11 @@ class _StepScorer:
             score(chunk, weights, sums[done:done + planes], self._workspace)
             done += planes
         self._rows += rows
+        self._used += len(rows) * width
 
     def _host_sums(self) -> np.ndarray:
-        n = len(self._rows)
-        return self._sums[:n].cpu().numpy() if n else np.zeros((0, self._SUMS))
+        """Every value accumulated so far, flat, in one device-to-host copy."""
+        return self._sums[:self._used].cpu().numpy() if self._used else np.zeros(0)
 
 
 class Scorer(_StepScorer):
@@ -316,7 +322,7 @@ class Scorer(_StepScorer):
         import pandas as pd
 
         n = len(self._rows)
-        s = self._host_sums()
+        s = self._host_sums().reshape(-1, self._SUMS)
         time, step, member, variable, level, has_clim = zip(*self._rows) if n else ((),) * 6
         with np.errstate(divide="ignore", invalid="ignore"):
             w = s[:, 0]
@@ -437,7 +443,7 @@ class EnsembleScorer(_StepScorer):
         import pandas as pd
 
         n = len(self._rows)
-        s = self._host_sums()
+        s = self._host_sums().reshape(-1, self._SUMS)
         time, step, variable, level, members, has_clim = zip(*self._rows) if n else ((),) * 6
         m = np.asarray(members, dtype=np.float64)
         with np.errstate(divide="ignore", invalid="ignore"):

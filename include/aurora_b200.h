@@ -543,6 +543,45 @@ int ab_ensemble_score_fields(const AbEnsembleField* fields, int32_t n_fields, si
                              const double* row_weights, double* sums, void* workspace, size_t workspace_bytes,
                              void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Latitude-band zonal power spectra of device-resident fields: for every level plane of every field and every band,
+ * the latitude-weighted mean over the band's rows of each row's one-sided variance spectrum, in one call.  Not a
+ * reference function: the reference's notebooks copy each prediction to the host and use numpy.fft.
+ *
+ * One AbSpectrumField per variable (and batch member): `levels` planes of h x w float32 values, row pitch ld,
+ * `level_stride` elements between planes; every field of a call has the same h and w.  Planes are numbered field by
+ * field, level by level.  Band b is the rows [band_rows[2b], band_rows[2b + 1]) (a HOST array).  For a row x_0..x_{N-1}
+ * (N = w), X_k = sum_n x_n e^{-2 pi i k n / N} in double and P(k) = c_k |X_k|^2 / N^2 for k = 0..N/2, c_k = 1 for
+ * k = 0 and (N even) k = N/2, else 2, so that sum_k P(k) = (1/N) sum_n x_n^2.  A row counts when all its N values are
+ * finite.  With w_r = row_weights[r] (double [h], DEVICE memory), out[p][b][0..N/2+2] =
+ *   sum w_r,  rows,  sum w_r P_r(0),  ...,  sum w_r P_r(N/2)
+ * over the counted rows of band b of plane p.  Each row is staged in shared memory (cp.async.bulk where the row
+ * address and 4 w bytes are 16-byte multiples, cp.async otherwise) and transformed two rows at a time as one complex
+ * mixed-radix (4 / 2 / 3 / 5) FFT in double.  Rows are split into a fixed (plane, band, row-chunk) partition whose
+ * partial sums go to `workspace` and are added in a fixed order by a second launch, so repeated calls give
+ * bit-identical sums (no atomics).  `fields` is a HOST array copied into the launch; `field_bytes` must be
+ * sizeof(AbSpectrumField); 0 <= n_fields <= AB_SPEC_MAX_FIELDS (0 is a no-op); 1 <= n_bands <= AB_SPEC_MAX_BANDS;
+ * 0 <= band_rows[2b] <= band_rows[2b + 1] <= h; h, levels >= 1; 1 <= w <= AB_SPEC_MAX_WIDTH with no prime factor
+ * above 5; ld >= w, level_stride >= 0.  `out` is double [total planes][n_bands][w/2 + 3], DEVICE memory.
+ * ---------------------------------------------------------------------------------------------- */
+#define AB_SPEC_MAX_FIELDS 64 /* the 9 variables of the 1.3 B model for up to 7 members in one call */
+#define AB_SPEC_MAX_BANDS 8
+#define AB_SPEC_MAX_WIDTH 4096
+
+typedef struct AbSpectrumField {
+  const float* x;       /* f32 [levels][h, ld] */
+  int64_t level_stride; /* elements between consecutive levels */
+  int32_t h, w, ld;
+  int32_t levels;
+} AbSpectrumField;
+
+/* Workspace `ab_zonal_spectra` needs for these fields and bands (validates them like it does).  Host only. */
+int ab_zonal_spectra_workspace_bytes(const AbSpectrumField* fields, int32_t n_fields, size_t field_bytes,
+                                     const int32_t* band_rows, int32_t n_bands, size_t* bytes);
+int ab_zonal_spectra(const AbSpectrumField* fields, int32_t n_fields, size_t field_bytes, const int32_t* band_rows,
+                     int32_t n_bands, const double* row_weights, double* out, void* workspace, size_t workspace_bytes,
+                     void* stream);
+
 /* sizeof() of the descriptor structs as this library was compiled (binding authors: compare with your mirror).
  * which: 0 AbGemm, 1 AbWindowAttention, 2 AbLnModResidual, 3 AbFieldIn, 4 AbFieldOut, 5 AbHaloPush, 6 AbSwinBlock,
  * 7 AbGemmLn, 8 AbPatchMergeLn, 9 AbPatchSplitLn, 10 AbOp; -1 for an unknown index.  Host only. */
